@@ -774,23 +774,28 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return n;
   };
   int bx = 0;
-  if (const char* s = getenv("MPPIB_BX"))
+  const bool bx_set = getenv("MPPIB_BX") != nullptr;
+  if (bx_set)
   {
-    bx = atoi(s);
+    bx = atoi(getenv("MPPIB_BX"));
     if (bx < unit || bx > 512 || (bx % unit) != 0)
       bx = 0;
   }
+  int ws_one_wave = 0;  // warp-specialised kernel: the one-CTA-per-SM width, when __launch_bounds__ allows it
   if (bx == 0 && ws)
   {
     // warp-specialised kernel: up to one warp per scheduler, one pair per CTA (no two producers ever share a scheduler);
     // beyond that ONE CTA per SM, as narrow as covers n_local, so that every SM is busy and the kernel's alternating role
-    // table (P C C P C P P C) balances producers over the four schedulers. Wider than fits: the wave rule below.
+    // table (P C C P C P P C) balances producers over the four schedulers. Wider than the resident tile fits: the wave rule
+    // below, and then the streaming form at this width.
     const long pairs_total = (e->n_local + 31) / 32;
     if (ws_wpg * pairs_total <= 4L * num_sms)
       bx = 32;
     else
     {
       const int need = (int)(((e->n_local + num_sms - 1) / num_sms + 31) / 32) * 32;
+      if (need <= max_bx)
+        ws_one_wave = need;
       if (need <= max_bx && smem_for(need) <= max_smem)
         bx = need;
     }
@@ -879,6 +884,35 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
         e->writeback = true;
       bx = sbx;
       e->smem_bytes = (uint32_t)sm_str;
+    }
+  }
+  // warp-specialised K1, streaming form (rollout_kernel_ar_ws.cuh: STREAM), by the same rule at the one-CTA-per-SM width:
+  // chosen when the resident tile needs several waves and the ring fits in fewer. On 132 SMs that is C4 (N = 32768: the
+  // 256-sample resident tile does not fit, and the 96-thread CTAs the wave rule falls back to run in two waves).
+  // MPPIB_STREAM=0/1 overrides; forced, it also runs without TMA (the issuing warp fills the ring with plain loads).
+  if (ws)
+  {
+    const bool tma_ok = !(desc->flags & MPPIB_FLAG_NO_TMA) && (e->TC % 4 == 0) && !getenv("MPPIB_NO_TMA");
+    const int sbx = (ws_one_wave && !bx_set) ? ws_one_wave : bx;
+    const int sm_str = (int)rollout_smem_layout(sbx, ar_ws::kNoiseRing, 1, e->TC, ar_ws::sharedFloats(sbx),
+                                                e->cost_shared_floats(e->T))
+                           .total;
+    if (sm_str <= max_smem)
+    {
+      auto waves = [&](int b, int sm) {
+        const long per_wave = (long)std::max(1, ctas_per_sm(b, sm)) * num_sms;
+        return ((e->n_local + b - 1) / b + per_wave - 1) / per_wave;
+      };
+      const long waves_res = waves(bx, smem_for(bx));
+      bool want = tma_ok && e->nchunks > ar_ws::kNoiseRing && waves_res > 1 && waves(sbx, sm_str) < waves_res;
+      if (const char* sv = getenv("MPPIB_STREAM"))
+        want = atoi(sv) != 0;
+      if (want)
+      {
+        e->stream_k1 = true;
+        bx = sbx;
+        e->smem_bytes = (uint32_t)sm_str;
+      }
     }
   }
   e->bx = bx;

@@ -322,6 +322,13 @@ struct Pair
                                                 std::is_same<COST, plugins::ARStandardCost>::value;
   static constexpr bool kHasWarpSpecVariant = std::is_same<DYN, plugins::AutorallyNNMmaDynamics<32>>::value &&
                                               std::is_same<COST, plugins::ARStandardCost>::value;
+  // the warp-specialised K1 the engine runs (samples per producer warp, write-back, streaming form)
+  static ArWsKernel ar_ws_kernel(const mppib_engine& e)
+  {
+    const bool wb = e.writeback, st = e.stream_k1;
+    return e.ws_pspw == 16 ? ar_ws_kernel_for<16>(wb, st)
+                           : (e.ws_pspw == 8 ? ar_ws_kernel_for<8>(wb, st) : ar_ws_kernel_for<32>(wb, st));
+  }
   static int prepare(mppib_engine& e)
   {
     if constexpr (kHasTensorCoreVariant)
@@ -341,18 +348,7 @@ struct Pair
     {
       if (e.ar_ws)
       {
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<true, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<false, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<true, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
-        CUDA_TRY(cudaFuncSetAttribute(rollout_kernel_ar_ws<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)e.smem_bytes));
+        CUDA_TRY(cudaFuncSetAttribute(ar_ws_kernel(e), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e.smem_bytes));
         return MPPIB_OK;
       }
     }
@@ -458,24 +454,7 @@ struct Pair
       if (e.ar_ws)
       {
         const int ws_threads = e.bx * ar_ws::warpsPerGroup(e.ws_pspw);
-        if (e.ws_pspw == 16)
-        {
-          if (e.writeback)
-            rollout_kernel_ar_ws<true, 16><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
-          else
-            rollout_kernel_ar_ws<false, 16><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
-        }
-        else if (e.ws_pspw == 8)
-        {
-          if (e.writeback)
-            rollout_kernel_ar_ws<true, 8><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
-          else
-            rollout_kernel_ar_ws<false, 8><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
-        }
-        else if (e.writeback)
-          rollout_kernel_ar_ws<true, 32><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
-        else
-          rollout_kernel_ar_ws<false, 32><<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
+        ar_ws_kernel(e)<<<e.grid, ws_threads, e.smem_bytes, e.stream>>>(a, e.tmap);
         launched = true;
       }
     }

@@ -106,6 +106,69 @@ __device__ __forceinline__ float likelihood_ratio_cost(const float* lr_scale, co
   return half_lambda_1ma * cost;
 }
 
+// The block epilogue's exp-weighted sum of the constrained controls of step t (weightedReductionKernel, mppi_common.cu:710-737)
+// over the block's rows [r_lo, r_hi), added to acc in row order. The value of a row comes from the shared tile (`slab` = the
+// step's column in its slab, `grp` its 16-byte group) or, from_global, from gsrc ([n_local][T][C]); `recompute`: that value is
+// noise and the constrained control is formed from it as the rollout did. Rows in blocks of 8 (r_lo a multiple of 8): the
+// swizzle term (grp ^ (r & 7)) << 4 is then a per-lane constant of the unrolled body. The loads of a block are issued first and
+// unconditionally (rows past r_hi are clamped and get weight 0), so eight loads are in flight per thread instead of one
+// load-use round trip per row — when they read L2 / HBM a serialised loop would expose one memory latency per row.
+template <class DYN, class ARGS>
+__device__ __forceinline__ void weighted_control_rows(const ARGS& args, int d, int t, int row0, int r_lo, int r_hi,
+                                                      const unsigned char* slab, int grp, const float* mean_t,
+                                                      bool t_uses_mean, const float* wrow, bool from_global,
+                                                      const float* gsrc, bool recompute, float* acc)
+{
+  constexpr int C = DYN::CONTROL_DIM;
+  const int T = args.T;
+  for (int r8 = r_lo; r8 < r_hi; r8 += 8)
+  {
+    float v[8][C];
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+    {
+      const int r = min(r8 + i, r_hi - 1);
+      if (from_global)
+      {
+        const float* q = gsrc + ((size_t)(row0 + r) * T + t) * C;
+#pragma unroll
+        for (int c = 0; c < C; c++)
+          v[i][c] = __ldg(q + c);
+      }
+      else
+      {
+        const float* p = reinterpret_cast<const float*>(slab + r * kChunkBytes + ((grp ^ (r & 7)) << 4));
+#pragma unroll
+        for (int c = 0; c < C; c++)
+          v[i][c] = p[c];
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+    {
+      const int r = r8 + i;
+      float u[C];
+#pragma unroll
+      for (int c = 0; c < C; c++)
+        u[c] = v[i][c];
+      if (recompute)
+      {
+        const int ng = args.n_offset + row0 + min(r, r_hi - 1);
+        const bool pn = (float)ng >= args.samp.pure_noise_threshold;
+        const bool um = t_uses_mean || (ng == 0);
+#pragma unroll
+        for (int c = 0; c < C; c++)
+          u[c] = sample_control(mean_t[c], args.samp.std_dev_decayed[d][c], v[i][c], um, pn);
+        DYN::enforceConstraints(args.dyn, nullptr, u);
+      }
+      const float w = (r < r_hi) ? wrow[r] : 0.0f;
+#pragma unroll
+      for (int c = 0; c < C; c++)
+        acc[c] = fmaf(w, u[c], acc[c]);
+    }
+  }
+}
+
 // shared-memory carve-up (bytes); the tile base is rounded up to 1024 B inside the kernel (SWIZZLE_128B atom)
 struct RolloutSmem
 {
@@ -542,53 +605,11 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
       const bool from_global = (RMPPI && d == 1) || STREAM;
       const bool readback = (RMPPI && d == 1) || (STREAM && WRITEBACK && args.stream_readback);
       const float* gsrc = readback ? args.controls_out + (size_t)d * args.n_local * T * C : args.eps;
-      for (int r8 = 0; r8 < rows_here; r8 += 8)
-      {
-        float v[8][C];
-#pragma unroll
-        for (int i = 0; i < 8; i++)
-        {
-          const int r = min(r8 + i, rows_here - 1);
-          if (from_global)
-          {
-            const float* q = gsrc + ((size_t)(row0 + r) * T + t) * C;
-#pragma unroll
-            for (int c = 0; c < C; c++)
-              v[i][c] = __ldg(q + c);
-          }
-          else
-          {
-            const float* p = reinterpret_cast<const float*>(slab + r * kChunkBytes + ((grp ^ (r & 7)) << 4));
-#pragma unroll
-            for (int c = 0; c < C; c++)
-              v[i][c] = p[c];
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; i++)
-        {
-          const int r = r8 + i;
-          float u[C];
-#pragma unroll
-          for (int c = 0; c < C; c++)
-            u[c] = v[i][c];
-          if (!(D == 1 && !STREAM) && !readback)
-          {  // the value is noise: recompute the constrained control (resident tile with D == 2, or the streaming variant, whose
-             // ring no longer holds it: a second read of eps instead of a write + read of u)
-            const int ng = args.n_offset + row0 + min(r, rows_here - 1);
-            const bool pn = (float)ng >= args.samp.pure_noise_threshold;
-            const bool um = t_uses_mean || (ng == 0);
-#pragma unroll
-            for (int c = 0; c < C; c++)
-              u[c] = sample_control(mean_t[c], args.samp.std_dev_decayed[d][c], v[i][c], um, pn);
-            DYN::enforceConstraints(args.dyn, nullptr, u);
-          }
-          const float w = (r < rows_here) ? wrow[r] : 0.0f;
-#pragma unroll
-          for (int c = 0; c < C; c++)
-            acc[c] = fmaf(w, u[c], acc[c]);
-        }
-      }
+      // the value is noise unless it comes from the constrained tile or the written-back controls: recompute the constrained
+      // control (resident tile with D == 2, or the streaming variant, whose ring no longer holds it: a second read of eps
+      // instead of a write + read of u)
+      weighted_control_rows<DYN>(args, d, t, row0, 0, rows_here, slab, grp, mean_t, t_uses_mean, wrow, from_global, gsrc,
+                                 !(D == 1 && !STREAM) && !readback, acc);
 #pragma unroll
       for (int c = 0; c < C; c++)
         out[col + c] = acc[c];
