@@ -17,7 +17,7 @@
  *
  *   phase 0 (all warps)   noise tile -> constrained controls, in place in shared memory (what setGaussianControls +
  *                         enforceConstraints + writeControlSample do in HBM): no recurrence, fully parallel. Resident form
- *                         only; the streaming form (below, STREAM) forms the controls in the readers instead.
+ *                         only; in the streaming form (below, STREAM) the consumers form them two groups ahead.
  *   producer warp         32 / 16 / 8 samples' network recurrence and nothing else, ENTIRELY in mma fragment layout: lane (g, t)
  *                         keeps states (3 + 2t, 4 + 2t) of its rows g, g+8, ... (t < 2), reads those rows' controls
  *                         from the tile (t == 2), and the C fragment it gets back from layer 3 is exactly the derivative
@@ -112,9 +112,9 @@ __device__ __forceinline__ float4 group_controls(const ArWsArgs& args, const flo
 // Every buffer has a "full" barrier (TMA completion, or the issuing warp's plain loads) and an "empty" one that each warp of
 // the block arrives on once it has read its last group of the slab. One warp issues the refills: the consumer of group 0,
 // the lightest chain in the block. On entering slab k it waits until every warp has left slab k - 2 and refills that buffer
-// with slab k + 1. The slab stays raw noise: each reader forms the constrained controls it needs itself (producer control
-// lanes for their rows, the consumer for its row), with the same operations as phase 0, and the epilogue recomputes them
-// from a second read of eps (rollout_kernel.cuh, STREAM).
+// with slab k + 1. The consumers turn their rows' groups into constrained controls in place, kRing groups ahead, with the
+// same operations as phase 0 (controls_in_place below), and the epilogue recomputes them from a second read of eps
+// (rollout_kernel.cuh, STREAM).
 template <bool WRITEBACK, int PSPW, bool STREAM>
 __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
     rollout_kernel_ar_ws(const __grid_constant__ ArWsArgs args, const __grid_constant__ CUtensorMap tmap)
@@ -243,6 +243,23 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
   nn_mma::load_weights(args.dyn_aux.theta_d, theta_s);
   COST::initializeCosts(args.cost, args.cost_aux, theta_c, T);
   __syncthreads();
+  // streaming: noise group gi of block row r -> its constrained controls, in place in the ring (what phase 0 does for the
+  // resident tile). The consumer of a row does it for group gi + kRing before it frees ring slot gi, which is what lets the
+  // producers of that row start group gi + kRing, so the producers read finished controls; groups 0 .. kRing - 1 are done here.
+  auto controls_in_place = [&](int r, int gi) {
+    float4* p = reinterpret_cast<float4*>(tile + (size_t)((gi >> 3) % kNoiseRing) * slab_bytes + (uint32_t)r * kChunkBytes +
+                                          ((uint32_t)((gi & 7) ^ (r & 7)) << 4));
+    const int n_glob = args.n_offset + row0 + r;
+    *p = group_controls(args, means_s, *p, 2 * gi, n_glob == 0, (float)n_glob >= args.samp.pure_noise_threshold);
+  };
+  if (STREAM)
+  {
+    mbar_wait(&bars[0], 0);
+    for (int i = thr; i < bx * kRing; i += nthr)
+      if (4 * (i % kRing) < TC)
+        controls_in_place(i / kRing, i % kRing);
+    __syncthreads();
+  }
 
   // ---- phase 0 (resident tile): noise -> constrained controls, in place (mppi_common.cu:117) --------------------------
   if (!STREAM)
@@ -325,6 +342,8 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
       if (STREAM && gg == 0)
         mbar_wait(&bars[k % kNoiseRing], (k / kNoiseRing) & 1);
       const unsigned char* slab = tile + (size_t)(STREAM ? k % kNoiseRing : k) * slab_bytes;
+      const int slot = gi % kRing;
+      mbar_wait(&empty[slot], (((unsigned)gi / kRing) & 1u) ^ 1u);  // streaming: also, the consumer has formed group gi
       float4 uu[NR];
 #pragma unroll
       for (int j = 0; j < NR; j++)
@@ -335,8 +354,6 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
         if (lane == 0)
           mbar_arrive(&slab_empty[k % kNoiseRing]);
       }
-      const int slot = gi % kRing;
-      mbar_wait(&empty[slot], (((unsigned)gi / kRing) & 1u) ^ 1u);
       float* out = ring + slot * kSlotFloats;
 #pragma unroll 1
       for (int s = 0; s < 2; s++)
@@ -349,12 +366,7 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
 #pragma unroll
         for (int j = 0; j < NR; j++)
         {
-          float2 uv = s == 0 ? make_float2(uu[j].x, uu[j].y) : make_float2(uu[j].z, uu[j].w);
-          if (STREAM)
-          {  // raw noise: the control lanes form the constrained control of their row
-            const int n_glob = args.n_offset + row0 + (int)(roff[j] / kChunkBytes);
-            uv = step_controls(args, means_s, uv, gi * 2 + s, n_glob == 0, (float)n_glob >= args.samp.pure_noise_threshold);
-          }
+          const float2 uv = s == 0 ? make_float2(uu[j].x, uu[j].y) : make_float2(uu[j].z, uu[j].w);
           const float2 v = ctl_lane ? uv : st[j];
           nn_mma::split2(v.x, v.y, a_hi[j >> 1][j & 1], a_lo[j >> 1][j & 1]);
         }
@@ -428,7 +440,6 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
       float4 uu = *reinterpret_cast<const float4*>(slab + roff + (((uint32_t)gg ^ swz) << 4));
       if (STREAM)
       {
-        uu = group_controls(args, means_s, uu, 2 * gi, n_glob == 0, pure_noise);
         if (gg == 7 || gi == ngroups - 1)
         {
           __syncwarp();
@@ -447,6 +458,13 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
       mbar_wait(&full[slot], ((unsigned)gi / kRing) & 1u);
       const float4* in = reinterpret_cast<const float4*>(ring + slot * kSlotFloats);
       const float4 xs0 = in[lane], xs1 = in[32 + lane];
+      if (STREAM && gi + kRing < ngroups)
+      {  // the producers of this row may start group gi + kRing once slot gi is free: form its controls first
+        const int k2 = (gi + kRing) >> 3;
+        if (k2 != k)
+          mbar_wait(&bars[k2 % kNoiseRing], (k2 / kNoiseRing) & 1);
+        controls_in_place(row, gi + kRing);
+      }
       __syncwarp();
       if (lane == 0)
         mbar_arrive(&empty[slot]);
