@@ -224,6 +224,24 @@ int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* fe
 int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides, int num_candidates,
                     int samples_per_candidate, const float* U_nominal, int optimization_stride, float* costs_out);
 
+/* ---- DDP feedback (Tube-MPPI / RMPPI ancillary controller) ----------------------------------------------------- */
+/* DDPFeedback::setParams (feedback_controllers/DDP/ddp.cu:69-76) with DDPParams (DDP/ddp.cuh:16-26): tracking weights
+ * Q [S][S], Q_f [S][S], R [C][C] (row-major) and the iteration count. Until called: Q = Q_f = I, R = I, 1 iteration. */
+int mppib_set_ddp(mppib_engine* e, const float* Q, const float* Q_f, const float* R, int num_iterations);
+/* DDPFeedback::computeFeedback (ddp.cu:80-118): DDP::run (ddp/ddp.h:56-168) from x0 [S] around the targets x_target [T][S],
+ * u_target [T][C] (also the initial controls), with the engine's dt, the model's control ranges and the weights of
+ * mppib_set_ddp. One CTA on the engine's stream; T is independent of the engine's horizon. Outputs (each may be NULL):
+ *   gains [T][S][C]         fb_gain_traj_: K_t, C x S column-major per step; K_{T-1} = 0
+ *   x_out [T][S], u_out [T][C]   the final state / control trajectory (result_.state_trajectory / control_trajectory)
+ *   jac_out [T][S][S+C]     [A | B] = d f / d(x, u) of the model's computeGrad at the trajectory the last backward pass
+ *                           linearised around (df = I + dt [A | B])
+ * to_rmppi = 1 (engines with MPPIB_FLAG_RMPPI, T == the horizon): the kernel also writes the gains into the engine's
+ * feedback-gain buffer, so the next RMPPI solve applies them with no host copy (robust_mppi_controller.cu:629-632).
+ * MPPIB_ERR_UNSUPPORTED for dynamics without an analytic Jacobian (the RACER LSTM pair, plugins). A failed LDLT of Q_uu
+ * (the reference exits, ddp.h:112-116) returns MPPIB_ERR_INVALID_ARG and leaves every gain buffer untouched. */
+int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_target, const float* u_target, int to_rmppi,
+                       float* gains, float* x_out, float* u_out, float* jac_out);
+
 /* ---- sampled (visualisation) trajectories ---------------------------------------------------------------------- */
 /* VanillaMPPIController::calculateSampledStateTrajectories (controllers/MPPI/mppi_controller.cu:262-298) /
  * launchVisualizeKernel (core/mppi_common.cu:364-520, 1376-1420): after a solve, re-rolls the rollouts the host picked

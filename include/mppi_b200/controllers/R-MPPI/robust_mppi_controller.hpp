@@ -4,8 +4,12 @@
  * the candidate line search runs through mppib_init_eval (computeNominalStateAndStride, :571-617) and the host logic
  * (line-search weights, candidates, strides, best index) through the library's host twins.
  *
- * The DDP feedback controller is out of scope (SURVEY §8): FB_T is carried as a type only and its product — the gain
- * trajectory — is an input (setFeedbackGains). With no gains set the real system runs without feedback.
+ * Feedback: after initFeedback() (FB_T = DDPFeedback) every updateImportanceSamplingControl runs the DDP solve from the
+ * real state around the nominal trajectory (robust_mppi_controller.cu:546-568, 629-632); the kernel writes the gains
+ * straight into the engine's feedback buffer, which the next solve applies. Without it the gain trajectory is an input
+ * (setFeedbackGains; explicit gains switch the computation off until initFeedback() is called again). With no gains at
+ * all the real system runs without feedback. Like the reference's rollout, which always reads its feedback controller's
+ * device gains, disableFeedbackController() stops the recomputation and leaves the last gains applied.
  */
 #pragma once
 #include <cstring>
@@ -109,6 +113,7 @@ public:
   // the DDP gain trajectory: gains[t] = K_t (C x S); no gains => no feedback
   void setFeedbackGains(const std::vector<feedback_gain_matrix>& gains)
   {
+    this->enable_feedback_ = false;
     const int T = this->getNumTimesteps();
     fb_gains_.assign((size_t)T * DYN_T::STATE_DIM * DYN_T::CONTROL_DIM, 0.0f);
     for (int t = 0; t < T && t < (int)gains.size(); t++)
@@ -147,6 +152,28 @@ public:
     this->slideControlSequenceHelper(nominal_stride_, nominal_control_trajectory_);
     output_trajectory out = output_trajectory::Zero();
     this->computeOutputTrajectoryHelper(out, nominal_state_trajectory_, nominal_state_, nominal_control_trajectory_);
+    computeNominalFeedbackGains(state);
+  }
+  // robust_mppi_controller.cu:629-632
+  void computeNominalFeedbackGains(const Eigen::Ref<const state_array>& state)
+  {
+    computeFeedbackHelper(state, nominal_state_trajectory_, nominal_control_trajectory_);
+  }
+  // the gains go straight into the engine's feedback buffer (mppib_ddp_feedback with to_rmppi); the host copy is kept so a
+  // re-created engine gets them back
+  void computeFeedbackHelper(const Eigen::Ref<const state_array>& state, const Eigen::Ref<const state_trajectory>& state_traj,
+                             const Eigen::Ref<const control_trajectory>& control_traj) override
+  {
+    if (!this->enable_feedback_)
+      return;
+    this->runFeedback(state, state_traj, control_traj, true);
+    if constexpr (PARENT_CLASS::kHasDDPFeedback)
+      fb_gains_ = this->fb_controller_->getFeedbackState().fb_gain_traj_;
+    fb_gains_.resize((size_t)this->getNumTimesteps() * DYN_T::STATE_DIM * DYN_T::CONTROL_DIM);
+  }
+  // robust_mppi_controller.cuh: a no-op; the gains are computed in updateImportanceSamplingControl
+  void computeFeedback(const Eigen::Ref<const state_array>& /*state*/) override
+  {
   }
   // robust_mppi_controller.cu:571-617
   void computeNominalStateAndStride(const Eigen::Ref<const state_array>& state, int stride)

@@ -157,6 +157,17 @@ public:
       m.d_[i] = v;
     return m;
   }
+  static Matrix Identity()
+  {
+    Matrix m = Zero();
+    for (int i = 0; i < R && i < C; i++)
+      m.d_[i + i * R] = 1.0f;
+    return m;
+  }
+  void setIdentity()
+  {
+    *this = Identity();
+  }
   void setZero()
   {
     memset(d_, 0, sizeof(d_));
@@ -274,6 +285,36 @@ public:
   {
     d_[0] = v;
     return CommaInit{ *this, 1 };
+  }
+  // m.diagonal() << a, b, c;  (the reference's examples set DDP weights this way)
+  struct DiagonalInit
+  {
+    Matrix& m;
+    int k;
+    DiagonalInit& operator,(float v)
+    {
+      assert(k < (R < C ? R : C));
+      m.d_[k + k * R] = v;
+      k++;
+      return *this;
+    }
+  };
+  struct Diagonal
+  {
+    Matrix& m;
+    DiagonalInit operator<<(float v)
+    {
+      m.d_[0] = v;
+      return DiagonalInit{ m, 1 };
+    }
+    float operator()(int i) const
+    {
+      return m.d_[i + i * R];
+    }
+  };
+  Diagonal diagonal()
+  {
+    return Diagonal{ *this };
   }
 
 private:

@@ -683,6 +683,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   e->init_eval = entry->init_eval;
   e->sampled_traj = entry->sampled_traj;
   e->nominal_traj = entry->nominal_traj;
+  e->ddp = entry->ddp;
   e->dyn_param_bytes = entry->dyn_bytes;
   e->cost_param_bytes = entry->cost_bytes;
   e->dyn_shared_floats_fn = entry->dyn_shared_floats;
@@ -1125,6 +1126,8 @@ int mppib_destroy(mppib_engine* e)
   cudaFree(e->lstm_theta_d);
   cudaFree(e->elev_d);
   cudaFree(e->fb_gains_d);
+  cudaFree(e->ddp_ws_d);
+  cudaFree(e->ddp_status_d);
   cudaFree(e->eval_states_d);
   cudaFree(e->eval_strides_d);
   cudaFree(e->eval_costs_d);
@@ -1812,6 +1815,102 @@ int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* fe
     cudaFree(e->fb_gains_d);
     e->fb_gains_d = nullptr;
   }
+  return MPPIB_OK;
+}
+
+int mppib_set_ddp(mppib_engine* e, const float* Q, const float* Q_f, const float* R, int num_iterations)
+{
+  if (!e || !Q || !Q_f || !R)
+    return fail(MPPIB_ERR_INVALID_ARG, "null argument");
+  if (num_iterations < 1)
+    return fail(MPPIB_ERR_INVALID_ARG, "num_iterations must be >= 1 (got %d)", num_iterations);
+  const int S = e->S, C = e->C;
+  for (int i = 0; i < S * S; i++)
+    if (!std::isfinite(Q[i]) || !std::isfinite(Q_f[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight Q / Q_f entry %d is not finite", i);
+  for (int i = 0; i < C * C; i++)
+    if (!std::isfinite(R[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight R entry %d is not finite", i);
+  e->ddp_Q.assign(Q, Q + S * S);
+  e->ddp_Qf.assign(Q_f, Q_f + S * S);
+  e->ddp_R.assign(R, R + C * C);
+  e->ddp_iters = num_iterations;
+  return MPPIB_OK;
+}
+
+int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_target, const float* u_target, int to_rmppi,
+                       float* gains, float* x_out, float* u_out, float* jac_out)
+{
+  if (!e || !x0 || !x_target || !u_target)
+    return fail(MPPIB_ERR_INVALID_ARG, "null argument");
+  if (!e->ddp)
+    return fail(MPPIB_ERR_UNSUPPORTED, "dynamics %d has no analytic Jacobian (computeGrad): no DDP kernel is built for it",
+                e->desc.dynamics_id);
+  if (T < 2)
+    return fail(MPPIB_ERR_INVALID_ARG, "DDP needs num_timesteps >= 2 (got %d)", T);
+  if (to_rmppi && !e->rmppi)
+    return fail(MPPIB_ERR_INVALID_ARG, "to_rmppi needs an engine created with MPPIB_FLAG_RMPPI");
+  if (to_rmppi && T != e->T)
+    return fail(MPPIB_ERR_INVALID_ARG, "to_rmppi needs T == the engine's horizon %d (got %d)", e->T, T);
+  if (!e->have_dyn)
+    return fail(MPPIB_ERR_STATE, "dynamics parameters were not set");
+  if (e->desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && !e->nn_theta_d)
+    return fail(MPPIB_ERR_STATE, "network weights were not set");
+  if (e->pending != 0)
+    return fail(MPPIB_ERR_STATE, "mppib_ddp_feedback while a solve is pending: call mppib_solve_wait first");
+  const int S = e->S, C = e->C;
+  for (int i = 0; i < S; i++)
+    if (!std::isfinite(x0[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "x0[%d] is not finite", i);
+  for (size_t i = 0; i < (size_t)T * S; i++)
+    if (!std::isfinite(x_target[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "x_target entry %zu is not finite", i);
+  for (size_t i = 0; i < (size_t)T * C; i++)
+    if (!std::isfinite(u_target[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "u_target entry %zu is not finite", i);
+  CUDA_TRY(cudaSetDevice(e->desc.device));
+  if (T > e->ddp_capacity)
+  {
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
+    cudaFree(e->ddp_ws_d);
+    e->ddp_ws_d = nullptr;
+    e->ddp_capacity = 0;
+    CUDA_TRY(cudaMalloc(&e->ddp_ws_d, ddp::ws_layout(T, S, C).total * sizeof(float)));
+    e->ddp_capacity = T;
+  }
+  if (!e->ddp_status_d)
+    CUDA_TRY(cudaMalloc(&e->ddp_status_d, sizeof(int)));
+  if (to_rmppi && !e->fb_gains_d)
+  {
+    CUDA_TRY(cudaMalloc(&e->fb_gains_d, (size_t)T * S * C * sizeof(float)));
+    CUDA_TRY(cudaMemsetAsync(e->fb_gains_d, 0, (size_t)T * S * C * sizeof(float), e->stream));
+  }
+  const ddp::WsLayout L = ddp::ws_layout(T, S, C);
+  float* ws = e->ddp_ws_d;
+  CUDA_TRY(cudaMemcpyAsync(ws + L.xt, x_target, (size_t)T * S * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+  CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+  // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
+  CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+  int rc = e->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d : nullptr);
+  if (rc != MPPIB_OK)
+    return rc;
+  int status = 0;
+  CUDA_TRY(cudaMemcpyAsync(&status, e->ddp_status_d, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+  CUDA_TRY(cudaStreamSynchronize(e->stream));
+  if (status != 0)
+    return fail(MPPIB_ERR_INVALID_ARG, "DDP: the LDLT of Q_uu failed at step %d (the reference exits, ddp.h:112-116); "
+                                       "gains left unchanged", status - 1);
+  if (gains)
+    CUDA_TRY(cudaMemcpyAsync(gains, ws + L.K, (size_t)T * S * C * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  if (x_out)
+    CUDA_TRY(cudaMemcpyAsync(x_out, ws + L.x, (size_t)T * S * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  if (u_out)
+    CUDA_TRY(cudaMemcpyAsync(u_out, ws + L.u, (size_t)T * C * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+  if (jac_out)
+    CUDA_TRY(cudaMemcpyAsync(jac_out, ws + L.jac, (size_t)T * S * (S + C) * sizeof(float), cudaMemcpyDeviceToHost,
+                             e->stream));
+  if (gains || x_out || u_out || jac_out)
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
   return MPPIB_OK;
 }
 

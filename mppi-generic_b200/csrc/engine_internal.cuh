@@ -26,6 +26,7 @@
 
 #include "../../include/mppi_b200.h"
 #include "combine_kernel.cuh"
+#include "ddp_kernel.cuh"
 #include "plugins/costs.cuh"
 #include "plugins/dynamics.cuh"
 #include "rollout_kernel.cuh"
@@ -110,6 +111,14 @@ struct mppib_engine
   int* vis_crash_d = nullptr;
   int vis_capacity = 0;
   int (*sampled_traj)(mppib_engine&, const float*, const float*, int, int, bool) = nullptr;
+  // DDP feedback (ddp_kernel.cuh, mppib_set_ddp / mppib_ddp_feedback): weights (empty = identity, DDPParams defaults), the
+  // workspace sized for ddp_capacity steps, the solve's status word, and the pair's launcher (null: no analytic Jacobian)
+  std::vector<float> ddp_Q, ddp_Qf, ddp_R;
+  int ddp_iters = 1;
+  float* ddp_ws_d = nullptr;
+  int* ddp_status_d = nullptr;
+  int ddp_capacity = 0;
+  int (*ddp)(mppib_engine&, int T, const float* x0, float* gains_d) = nullptr;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
 
@@ -637,6 +646,49 @@ static int nominal_traj_launch(mppib_engine& e, const float* x0, const float* u_
   return MPPIB_OK;
 }
 
+// DDPFeedback::computeFeedback for this pair's dynamics (ddp_kernel.cuh): the workspace already holds the targets and the
+// initial controls; gains_d = the destination of the gain trajectory, or null
+template <class DYN>
+static int ddp_launch(mppib_engine& e, int T, const float* x0, float* gains_d)
+{
+  using Args = ddp::DdpArgs<DYN>;
+  constexpr int S = DYN::STATE_DIM, C = DYN::CONTROL_DIM;
+  static_assert(sizeof(Args) < 4000, "kernel parameter block too large");
+  Args a;
+  memcpy(&a.dyn, e.dyn_blob.data(), sizeof(a.dyn));
+  AuxFill<typename DYN::Aux>::fill(a.aux, e);
+  for (int i = 0; i < S * S; i++)
+  {
+    a.Q[i] = e.ddp_Q.empty() ? (i % (S + 1) == 0 ? 1.0f : 0.0f) : e.ddp_Q[i];
+    a.Qf[i] = e.ddp_Qf.empty() ? (i % (S + 1) == 0 ? 1.0f : 0.0f) : e.ddp_Qf[i];
+  }
+  for (int i = 0; i < C * C; i++)
+    a.R[i] = e.ddp_R.empty() ? (i % (C + 1) == 0 ? 1.0f : 0.0f) : e.ddp_R[i];
+  memcpy(a.x0, x0, sizeof(a.x0));
+  for (int c = 0; c < C; c++)
+  {
+    a.u_lo[c] = a.dyn.lim.rng_lo[c];
+    a.u_hi[c] = a.dyn.lim.rng_hi[c];
+  }
+  a.dt = e.dt;
+  a.T = T;
+  a.iters = e.ddp_iters;
+  a.ws = e.ddp_ws_d;
+  a.gains = gains_d;
+  a.status = e.ddp_status_d;
+  ddp::ddp_kernel<DYN><<<1, ddp::kThreads, 0, e.stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  return MPPIB_OK;
+}
+template <class DYN>
+constexpr int (*ddp_launcher())(mppib_engine&, int, const float*, float*)
+{
+  if constexpr (DYN::HAS_GRAD)
+    return &ddp_launch<DYN>;
+  else
+    return nullptr;
+}
+
 struct PairEntry
 {
   int dyn_id, cost_id;
@@ -653,6 +705,7 @@ struct PairEntry
   int (*stream_blocks_per_sm)(int, int, size_t);
   int (*sampled_traj)(mppib_engine&, const float*, const float*, int, int, bool);
   int (*nominal_traj)(mppib_engine&, const float*, const float*, int, const float*);
+  int (*ddp)(mppib_engine&, int, const float*, float*);  // null: the dynamics have no analytic Jacobian (HAS_GRAD)
 };
 template <class DYN, class COST>
 constexpr PairEntry make_entry(int dyn_id, int cost_id)
@@ -674,7 +727,8 @@ constexpr PairEntry make_entry(int dyn_id, int cost_id)
                     &init_eval_launch<typename DYN::AuxDyn, COST>,
                     &Pair<DYN, COST>::stream_blocks_per_sm,
                     &sampled_traj_launch<typename DYN::AuxDyn, COST>,
-                    &nominal_traj_launch<typename DYN::AuxDyn> };
+                    &nominal_traj_launch<typename DYN::AuxDyn>,
+                    ddp_launcher<typename DYN::AuxDyn>() };
 }
 
 // ---- registration of out-of-tree pairs -------------------------------------------------------------------------------------

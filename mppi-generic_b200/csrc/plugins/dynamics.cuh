@@ -61,6 +61,11 @@ struct Dynamics
   // step is warp-collective, plugins/nn_mma.cuh, shorten the per-warp chain this way when a GPU holds few rollouts)
   static constexpr int SAMPLES_PER_WARP = 32;
   using AuxDyn = CLASS_T;  // the form the one-thread-per-rollout auxiliary kernels (init-eval, sampled trajectories) instantiate
+  // the model has an analytic Jacobian, computeGrad(p, aux, x, u, A, B): A = df/dx [S][S], B = df/du [S][C], both row-major
+  // (Dynamics::computeGrad, dynamics.cuh:236-240). Only such models get the DDP feedback solver (ddp_kernel.cuh).
+  static constexpr bool HAS_GRAD = false;
+  // ddp_kernel.cuh evaluates f with the warp-cooperative network of AutorallyNNDynamics instead of computeStateDeriv
+  static constexpr bool DDP_WARP_NN = false;
   struct Aux
   {
   };
@@ -158,6 +163,31 @@ struct CartpoleDynamics : public Dynamics<CartpoleDynamics, mppib_cartpole_dyn_p
     state_der[3] = rcp_nr(l_p * denom) * (-force * cos_theta - m_p * l_p * MPPIB_SQ(theta_dot) * cos_theta * sin_theta -
                                           (m_c + m_p) * gravity_ * sin_theta);
   }
+
+  static constexpr bool HAS_GRAD = true;
+  // cartpole_dynamics.cu:10-45, term for term. In the exact derivative the second quotient of A(3, 2) has one more factor
+  // pole_length in its numerator; the two agree at pole_length == 1, the reference's default.
+  __device__ static bool computeGrad(const Params& p, const Aux&, const float* x, const float* u, float* A, float* B)
+  {
+    const float th = x[2], td = x[3], F = u[0];
+    const float s = sinf(th), c = cosf(th), mc = p.cart_mass, mp = p.pole_mass, l = p.pole_length, g = p.gravity;
+    const float den = mc + mp * s * s;
+    for (int i = 0; i < 16; i++)
+      A[i] = 0.0f;
+    for (int i = 0; i < 4; i++)
+      B[i] = 0.0f;
+    A[0 * 4 + 1] = 1.0f;
+    A[1 * 4 + 2] = (mp * c * (l * td * td + g * c) - g * mp * s * s) / den -
+                   (2 * mp * c * s * (F + mp * s * (l * td * td + g * c))) / (den * den);
+    A[1 * 4 + 3] = (2 * l * mp * td * s) / den;
+    A[2 * 4 + 3] = 1.0f;
+    A[3 * 4 + 2] = (F * s - g * c * (mp + mc) - l * mp * td * td * c * c + l * mp * td * td * s * s) / (l * den) +
+                   (2 * mp * c * s * (l * mp * c * s * td * td + F * c + g * s * (mp + mc))) / ((l * den) * (l * den));
+    A[3 * 4 + 3] = -(2 * mp * td * c * s) / den;
+    B[1] = 1.0f / den;
+    B[3] = -c / (l * den);
+    return true;
+  }
 };
 
 // ---- Double integrator: dynamics/double_integrator/di_dynamics.cu:46-53 -------------------------------------------
@@ -170,6 +200,21 @@ struct DoubleIntegratorDynamics : public Dynamics<DoubleIntegratorDynamics, mppi
     state_der[1] = state[3];
     state_der[2] = control[0];
     state_der[3] = control[1];
+  }
+
+  static constexpr bool HAS_GRAD = true;
+  // di_dynamics.cu:24-34
+  __device__ static bool computeGrad(const Params&, const Aux&, const float*, const float*, float* A, float* B)
+  {
+    for (int i = 0; i < 16; i++)
+      A[i] = 0.0f;
+    for (int i = 0; i < 8; i++)
+      B[i] = 0.0f;
+    A[0 * 4 + 2] = 1.0f;
+    A[1 * 4 + 3] = 1.0f;
+    B[2 * 2 + 0] = 1.0f;
+    B[3 * 2 + 1] = 1.0f;
+    return true;
   }
 };
 
@@ -345,6 +390,67 @@ struct AutorallyNNDynamics : public Dynamics<AutorallyNNDynamics, mppib_ar_nn_dy
     for (int i = 0; i < DYNAMICS_DIM; i++)
       state_der[i + (7 - DYNAMICS_DIM)] = a3[i];
   }
+
+  static constexpr bool HAS_GRAD = true;
+  static constexpr bool DDP_WARP_NN = true;
+  // NeuralNetModel::computeGrad (ar_nn_model.cu:63-86): the kinematic rows, then the network's input Jacobian by
+  // back-propagation through the two tanh layers (FNNHelper::computeGrad, fnn_helper.cu:312-347). One thread, weights read
+  // from the packed blob in global memory (W row-major out x in, then b, per layer).
+  __device__ static bool computeGrad(const Params&, const Aux& aux, const float* x, const float* u, float* A, float* B)
+  {
+    const float* g = aux.theta_d;
+    const float *W1 = g, *b1 = g + 192, *W2 = g + 224, *b2 = g + 1248, *W3 = g + 1280;
+    for (int i = 0; i < 49; i++)
+      A[i] = 0.0f;
+    for (int i = 0; i < 14; i++)
+      B[i] = 0.0f;
+    float sn, cs;
+    sincosf(x[2], &sn, &cs);
+    A[0 * 7 + 2] = -sn * x[4] - cs * x[5];
+    A[0 * 7 + 4] = cs;
+    A[0 * 7 + 5] = -sn;
+    A[1 * 7 + 2] = cs * x[4] - sn * x[5];
+    A[1 * 7 + 4] = sn;
+    A[1 * 7 + 5] = cs;
+    A[2 * 7 + 6] = -1.0f;
+    const float in[6] = { x[3], x[4], x[5], x[6], u[0], u[1] };
+    float a1[32], d1[32], d2[32];
+    for (int j = 0; j < 32; j++)
+    {
+      float z = 0.0f;
+      for (int k = 0; k < 6; k++)
+        z = fmaf(__ldg(W1 + j * 6 + k), in[k], z);
+      a1[j] = tanhf(z + __ldg(b1 + j));
+      d1[j] = 1.0f - a1[j] * a1[j];  // tanh_deriv
+    }
+    for (int j = 0; j < 32; j++)
+    {
+      float z = 0.0f;
+      for (int k = 0; k < 32; k++)
+        z = fmaf(__ldg(W2 + j * 32 + k), a1[k], z);
+      const float a2 = tanhf(z + __ldg(b2 + j));
+      d2[j] = 1.0f - a2 * a2;
+    }
+    for (int i = 0; i < 4; i++)
+    {
+      // row i of d out / d in = W3[i] diag(d2) W2 diag(d1) W1
+      float r[6] = { 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f };
+      for (int j = 0; j < 32; j++)
+      {
+        float gj = 0.0f;
+        for (int k = 0; k < 32; k++)
+          gj = fmaf(__ldg(W3 + i * 32 + k) * d2[k], __ldg(W2 + k * 32 + j), gj);
+        gj *= d1[j];
+        for (int m = 0; m < 6; m++)
+          r[m] = fmaf(gj, __ldg(W1 + j * 6 + m), r[m]);
+      }
+      for (int m = 0; m < 4; m++)
+        A[(3 + i) * 7 + 3 + m] = r[m];
+      B[(3 + i) * 2 + 0] = r[4];
+      B[(3 + i) * 2 + 1] = r[5];
+    }
+    return true;
+  }
   // The same dense layer for M samples of one thread: one weight row (LDS.128 quads, broadcast) feeds M * OUT/2 FFMA2s.
   // Per-neuron accumulation order unchanged (k ascending, bias last), so every sample's values are those of layer<>.
   template <int IN, int OUT, bool TANH_IN, int M>
@@ -478,6 +584,12 @@ struct AutorallyNNMmaDynamics : public Dynamics<AutorallyNNMmaDynamics<SPW>, mpp
   __device__ static __forceinline__ void computeKinematics(const Params& p, const float* state, float* state_der)
   {
     AutorallyNNDynamics::computeKinematics(p, state, state_der);
+  }
+  static constexpr bool HAS_GRAD = true;
+  static constexpr bool DDP_WARP_NN = true;
+  __device__ static bool computeGrad(const Params& p, const Aux& aux, const float* x, const float* u, float* A, float* B)
+  {
+    return AutorallyNNDynamics::computeGrad(p, aux, x, u, A, B);
   }
   // warp-collective: every lane of the warp calls it (the rollout kernels keep out-of-range rows running)
   __device__ static __forceinline__ void computeDynamics(const Params&, const float* theta_s, const float* state,
@@ -1162,6 +1274,51 @@ struct QuadrotorDynamics : public Dynamics<QuadrotorDynamics, mppib_quadrotor_dy
 #pragma unroll
     for (int i = 0; i < 4; i++)
       q[i] *= inv;
+  }
+
+  static constexpr bool HAS_GRAD = true;
+  // The exact Jacobian of computeDynamics above. The reference's QuadrotorDynamics::computeGrad (quadrotor_dynamics.cu:
+  // 35-68) leaves dv/dq and dq/d(q, w) as TODOs, puts dq/dw in B and returns false, so its DDP wrapper falls back to numeric
+  // differences of f (ddp_model_wrapper.h:83-95); this is the derivative those differences approximate.
+  __device__ static bool computeGrad(const Params& p, const Aux&, const float* x, const float* u, float* A, float* B)
+  {
+    for (int i = 0; i < 169; i++)
+      A[i] = 0.0f;
+    for (int i = 0; i < 52; i++)
+      B[i] = 0.0f;
+    const float* q = x + 6;
+    const float* w = x + 10;
+    const float a = u[3] / p.mass;
+    for (int i = 0; i < 3; i++)
+      A[i * 13 + 3 + i] = 1.0f;  // dpos/dv
+    // dv/dq: a * d(third column of Quat2DCM)/dq
+    const float dcm[3][4] = { { 2 * q[2], 2 * q[3], 2 * q[0], 2 * q[1] },
+                              { -2 * q[1], -2 * q[0], 2 * q[3], 2 * q[2] },
+                              { 2 * q[0], -2 * q[1], -2 * q[2], 2 * q[3] } };
+    for (int r = 0; r < 3; r++)
+      for (int j = 0; j < 4; j++)
+        A[(3 + r) * 13 + 6 + j] = a * dcm[r][j];
+    B[3 * 4 + 3] = 2 * (q[1] * q[3] + q[0] * q[2]) / p.mass;
+    B[4 * 4 + 3] = 2 * (q[2] * q[3] - q[0] * q[1]) / p.mass;
+    B[5 * 4 + 3] = (q[0] * q[0] - q[1] * q[1] - q[2] * q[2] + q[3] * q[3]) / p.mass;
+    // dq/dq and dq/dw of omega2edot
+    const float dqq[4][4] = { { 0, -w[0], -w[1], -w[2] }, { w[0], 0, w[2], -w[1] }, { w[1], -w[2], 0, w[0] },
+                              { w[2], w[1], -w[0], 0 } };
+    const float dqw[4][3] = { { -q[1], -q[2], -q[3] }, { q[0], -q[3], q[2] }, { q[3], q[0], -q[1] }, { -q[2], q[1], q[0] } };
+    for (int r = 0; r < 4; r++)
+    {
+      for (int j = 0; j < 4; j++)
+        A[(6 + r) * 13 + 6 + j] = 0.5f * dqq[r][j];
+      for (int j = 0; j < 3; j++)
+        A[(6 + r) * 13 + 10 + j] = 0.5f * dqw[r][j];
+    }
+    const float tau[3] = { p.tau_roll, p.tau_pitch, p.tau_yaw };
+    for (int i = 0; i < 3; i++)
+    {
+      A[(10 + i) * 13 + 10 + i] = -1.0f / tau[i];
+      B[(10 + i) * 4 + i] = 1.0f / tau[i];
+    }
+    return true;
   }
 };
 
