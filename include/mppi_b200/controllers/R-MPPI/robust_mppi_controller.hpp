@@ -137,6 +137,20 @@ public:
   {
     return candidate_free_energy_;
   }
+  // robust_mppi_controller.cu:758-762: |x_fb(0) - x_fb(1)| + |x_nom(0) - x_fb(0)| on the feedback-propagated and the
+  // nominal state trajectories (call computeFeedbackPropagatedStateSeq first)
+  float computeDF()
+  {
+    const state_trajectory fb = this->getFeedbackPropagatedStateSeq();
+    const state_trajectory nom = getTargetStateSeq();
+    float a = 0.0f, b = 0.0f;
+    for (int i = 0; i < DYN_T::STATE_DIM; i++)
+    {
+      a += (fb(i, 0) - fb(i, 1)) * (fb(i, 0) - fb(i, 1));
+      b += (nom(i, 0) - fb(i, 0)) * (nom(i, 0) - fb(i, 0));
+    }
+    return sqrtf(a) + sqrtf(b);
+  }
   int getBestIndex() const
   {
     return best_index_;

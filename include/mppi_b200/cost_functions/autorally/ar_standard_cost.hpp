@@ -32,20 +32,18 @@ struct ARStandardCostParams : public CostParams<2>
   }
 };
 
-class ARStandardCost : public MPPI_internal::Cost<ARStandardCost, ARStandardCostParams, mppib_ar_standard_cost_params,
-                                                  MPPIB_COST_AR_STANDARD>
+namespace MPPI_internal
+{
+// The map-owning part of the Autorally map costs (ARStandardCostImpl, ar_standard_cost.cu:35-204): the costmap, its
+// world->texture transform and the blob fields every map cost shares (mppib_ar_standard_cost_params, the prefix of each map
+// cost's blob). ARStandardCost and ARRobustCost differ only in their params, blob and cost id.
+template <class CLASS_T, class PARAMS_T, class BLOB_T, int COST_ID_V>
+class ARMapCost : public Cost<CLASS_T, PARAMS_T, BLOB_T, COST_ID_V>
 {
 public:
   const float FRONT_D = 0.5;
   const float BACK_D = -0.5;
   bool l1_cost_ = false;
-  ARStandardCost(cudaStream_t stream = 0)
-  {
-  }
-  std::string getCostFunctionName() const override
-  {
-    return "AutoRally standard cost function";
-  }
   int getWidth() const
   {
     return width_;
@@ -74,9 +72,9 @@ public:
     changeCostmapSize(int((x_max - x_min) * ppm), int((y_max - y_min) * ppm));
     for (int i = 0; i < width_ * height_; i++)
       track_costs_[i] = float4{ ch0[i], ch1 ? ch1[i] : 0.0f, ch2 ? ch2[i] : 0.0f, ch3 ? ch3[i] : 0.0f };
-    params_.r_c1 = float3{ 1.0f / (x_max - x_min), 0, 0 };
-    params_.r_c2 = float3{ 0, 1.0f / (y_max - y_min), 0 };
-    params_.trs = float3{ -x_min / (x_max - x_min), -y_min / (y_max - y_min), 1 };
+    this->params_.r_c1 = float3{ 1.0f / (x_max - x_min), 0, 0 };
+    this->params_.r_c2 = float3{ 0, 1.0f / (y_max - y_min), 0 };
+    this->params_.trs = float3{ -x_min / (x_max - x_min), -y_min / (y_max - y_min), 1 };
   }
   // ARStandardCostImpl::loadTrackData (ar_standard_cost.cu:85-142): npz with "xBounds", "yBounds", "pixelsPerMeter" and
   // "channel0".."channel3" (float32, row-major [height][width]); returns the CPU copy like the reference (empty on error)
@@ -115,9 +113,9 @@ public:
   }
   void updateTransform(const Eigen::Matrix3f& m, const Eigen::Vector3f& trs)
   {  // ar_standard_cost.cu:188-204
-    params_.r_c1 = float3{ m(0, 0), m(1, 0), m(2, 0) };
-    params_.r_c2 = float3{ m(0, 1), m(1, 1), m(2, 1) };
-    params_.trs = float3{ trs(0), trs(1), trs(2) };
+    this->params_.r_c1 = float3{ m(0, 0), m(1, 0), m(2, 0) };
+    this->params_.r_c2 = float3{ m(0, 1), m(1, 1), m(2, 1) };
+    this->params_.trs = float3{ trs(0), trs(1), trs(2) };
   }
   const float* costmap() const
   {
@@ -127,22 +125,23 @@ public:
   {
     return track_costs_.size() * sizeof(float4);
   }
-  mppib_ar_standard_cost_params blob() const
+  BLOB_T blob() const
   {
-    mppib_ar_standard_cost_params b{};
-    fillBase(b);
-    b.desired_speed = params_.desired_speed;
-    b.speed_coeff = params_.speed_coeff;
-    b.track_coeff = params_.track_coeff;
-    b.max_slip_ang = params_.max_slip_ang;
-    b.slip_coeff = params_.slip_coeff;
-    b.track_slop = params_.track_slop;
-    b.crash_coeff = params_.crash_coeff;
-    b.boundary_threshold = params_.boundary_threshold;
-    b.grid_res = params_.grid_res;
-    b.r_c1[0] = params_.r_c1.x, b.r_c1[1] = params_.r_c1.y, b.r_c1[2] = params_.r_c1.z;
-    b.r_c2[0] = params_.r_c2.x, b.r_c2[1] = params_.r_c2.y, b.r_c2[2] = params_.r_c2.z;
-    b.trs[0] = params_.trs.x, b.trs[1] = params_.trs.y, b.trs[2] = params_.trs.z;
+    BLOB_T b{};
+    const PARAMS_T& p = this->params_;
+    this->fillBase(b);
+    b.desired_speed = p.desired_speed;
+    b.speed_coeff = p.speed_coeff;
+    b.track_coeff = p.track_coeff;
+    b.max_slip_ang = p.max_slip_ang;
+    b.slip_coeff = p.slip_coeff;
+    b.track_slop = p.track_slop;
+    b.crash_coeff = p.crash_coeff;
+    b.boundary_threshold = p.boundary_threshold;
+    b.grid_res = p.grid_res;
+    b.r_c1[0] = p.r_c1.x, b.r_c1[1] = p.r_c1.y, b.r_c1[2] = p.r_c1.z;
+    b.r_c2[0] = p.r_c2.x, b.r_c2[1] = p.r_c2.y, b.r_c2[2] = p.r_c2.z;
+    b.trs[0] = p.trs.x, b.trs[1] = p.trs.y, b.trs[2] = p.trs.z;
     b.l1_cost = l1_cost_ ? 1 : 0;
     b.front_d = FRONT_D;
     b.back_d = BACK_D;
@@ -151,7 +150,21 @@ public:
     return b;
   }
 
-private:
+protected:
   int width_ = -1, height_ = -1;
   std::vector<float4> track_costs_;
+};
+}  // namespace MPPI_internal
+
+class ARStandardCost : public MPPI_internal::ARMapCost<ARStandardCost, ARStandardCostParams, mppib_ar_standard_cost_params,
+                                                       MPPIB_COST_AR_STANDARD>
+{
+public:
+  ARStandardCost(cudaStream_t stream = 0)
+  {
+  }
+  std::string getCostFunctionName() const override
+  {
+    return "AutoRally standard cost function";
+  }
 };

@@ -9,6 +9,7 @@
  *   mppib_host_step_lstm / mppib_host_output_trajectory_lstm   the same two for RacerDubinsElevationLSTMSteering
  *   mppib_host_free_energy          mppi::kernels::computeFreeEnergy      include/mppi/core/mppi_common.cu:1065-1081
  *   mppib_host_merge_records        (no reference counterpart: the log-sum-exp merge of rollout shards, SURVEY §8e)
+ *   mppib_host_state_cost           the robust costs' host computeStateCost / getStabilizingCost / getCostmapCost (below)
  * Arrays: u / history are [T][C] / [2][C] (== Eigen C x T / C x 2 column-major), states [T][S], outputs [T][O].
  */
 #ifndef MPPI_B200_HOST_TWINS_H_
@@ -87,6 +88,18 @@ int mppib_host_merge_records(const float* records, int nrec, int D, int TC, int 
  * order; up to 4 dimensions. out == NULL: only *count / shape4 / *ndim are filled. */
 int mppib_host_npz_read(const char* path, const char* name, float* out, size_t capacity, size_t* count, int* shape4,
                         int* ndim);
+/* Host bodies of the robust costs, which the reference calls directly (cost.computeStateCost(y, t, &crash),
+ * ARRobustCost::getStabilizingCost / getCostmapCost):
+ *   MPPIB_COST_DI_ROBUST  double_integrator_robust_cost.cu:41-69: the HOST constants (steep boundary 0.75, steep cost
+ *                         0.1 * crash_cost); the rollouts use the device body's 0.5 / 0.5 * crash_cost, as in the reference
+ *   MPPIB_COST_AR_ROBUST  ar_robust_cost.cu:13-132, host branch: cosf / sinf and the nearest texel (std::round after the
+ *                         clamps of :64-70); costmap = float4 per texel, row-major [map_height][map_width]
+ * `params` is the cost's parameter blob (params.h). Other cost ids: MPPIB_ERR_UNSUPPORTED. Neither cost reads t or crash. */
+int mppib_host_state_cost(int cost_id, const void* params, const float* costmap, const float* y, int t, int* crash,
+                          float* cost);
+int mppib_host_ar_robust_stabilizing_cost(const mppib_ar_robust_cost_params* params, const float* s, float* cost);
+int mppib_host_ar_robust_costmap_cost(const mppib_ar_robust_cost_params* params, const float* costmap, const float* s,
+                                      float* cost);
 #ifdef __cplusplus
 }
 #endif

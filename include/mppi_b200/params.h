@@ -35,6 +35,8 @@ enum mppib_cost_id
   MPPIB_COST_AR_STANDARD = 2,        /* cost_functions/autorally/ar_standard_cost.cuh */
   MPPIB_COST_RACER_QUADRATIC = 3,    /* ours (SURVEY §8d C5): quadratic on speed / yaw, documented in DESIGN.md */
   MPPIB_COST_QUADROTOR_QUADRATIC = 4, /* cost_functions/quadrotor/quadrotor_quadratic_cost.cuh */
+  MPPIB_COST_DI_ROBUST = 5,          /* cost_functions/double_integrator/double_integrator_robust_cost.cuh (circle params) */
+  MPPIB_COST_AR_ROBUST = 6,          /* cost_functions/autorally/ar_robust_cost.cuh */
   MPPIB_COST_COUNT
 };
 
@@ -196,6 +198,61 @@ typedef struct mppib_ar_standard_cost_params /* cost_functions/autorally/ar_stan
   int map_width;            /* texture width  (costmap travels as MPPIB_BLOB_COSTMAP, float4 per texel) */
   int map_height;           /* texture height */
 } mppib_ar_standard_cost_params;
+
+/* ARRobustCostParams (cost_functions/autorally/ar_robust_cost.cuh:6-29): every field of the standard blob, in the same order,
+ * then heading_coeff. The shared prefix is what the costmap upload (MPPIB_BLOB_COSTMAP reads map_width / map_height) and
+ * the map helpers read, so they take either blob. */
+typedef struct mppib_ar_robust_cost_params
+{
+  float control_cost_coeff[MPPIB_MAX_CONTROL_DIM]; /* 0, 0 */
+  float discount;           /* 1.0 */
+  float desired_speed;      /* -1: follow the map's speed channel (.z) */
+  float speed_coeff;        /* 20 */
+  float track_coeff;        /* 33 */
+  float max_slip_ang;       /* 1.5 */
+  float slip_coeff;         /* 0 */
+  float track_slop;         /* 0 */
+  float crash_coeff;        /* 125000 */
+  float boundary_threshold; /* 0.75 */
+  int grid_res;             /* 10 (unused on the path) */
+  float r_c1[3];
+  float r_c2[3];
+  float trs[3];
+  int l1_cost;              /* unused by this cost */
+  float front_d;            /* 0.5 */
+  float back_d;             /* -0.5 */
+  int map_width;
+  int map_height;
+  float heading_coeff;      /* 0 */
+} mppib_ar_robust_cost_params;
+
+#ifdef __cplusplus
+#include <stddef.h>
+#define MPPIB_AR_PREFIX_SAME(f) \
+  static_assert(offsetof(mppib_ar_robust_cost_params, f) == offsetof(mppib_ar_standard_cost_params, f), #f);
+MPPIB_AR_PREFIX_SAME(control_cost_coeff)
+MPPIB_AR_PREFIX_SAME(discount)
+MPPIB_AR_PREFIX_SAME(desired_speed)
+MPPIB_AR_PREFIX_SAME(speed_coeff)
+MPPIB_AR_PREFIX_SAME(track_coeff)
+MPPIB_AR_PREFIX_SAME(max_slip_ang)
+MPPIB_AR_PREFIX_SAME(slip_coeff)
+MPPIB_AR_PREFIX_SAME(track_slop)
+MPPIB_AR_PREFIX_SAME(crash_coeff)
+MPPIB_AR_PREFIX_SAME(boundary_threshold)
+MPPIB_AR_PREFIX_SAME(grid_res)
+MPPIB_AR_PREFIX_SAME(r_c1)
+MPPIB_AR_PREFIX_SAME(r_c2)
+MPPIB_AR_PREFIX_SAME(trs)
+MPPIB_AR_PREFIX_SAME(l1_cost)
+MPPIB_AR_PREFIX_SAME(front_d)
+MPPIB_AR_PREFIX_SAME(back_d)
+MPPIB_AR_PREFIX_SAME(map_width)
+MPPIB_AR_PREFIX_SAME(map_height)
+static_assert(offsetof(mppib_ar_robust_cost_params, heading_coeff) == sizeof(mppib_ar_standard_cost_params),
+              "heading_coeff follows the standard prefix");
+#undef MPPIB_AR_PREFIX_SAME
+#endif
 
 /* Quadratic tracking cost on the RACER output vector (ours: the RACER cost classes are not in the reference tree,
  * SURVEY §8d C5). cost = speed_coeff (y[VEL_B_X] - desired_speed)^2 + yaw_coeff angdist(y[YAW], desired_yaw)^2

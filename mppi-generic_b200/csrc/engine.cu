@@ -106,6 +106,9 @@ static const PairEntry kPairs[] = {
   make_entry<plugins::DoubleIntegratorDynamics, plugins::DoubleIntegratorCircleCost>(MPPIB_DYN_DOUBLE_INTEGRATOR,
                                                                                      MPPIB_COST_DI_CIRCLE),
   make_entry<plugins::AutorallyNNDynamics, plugins::ARStandardCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_STANDARD),
+  make_entry<plugins::DoubleIntegratorDynamics, plugins::DoubleIntegratorRobustCost>(MPPIB_DYN_DOUBLE_INTEGRATOR,
+                                                                                     MPPIB_COST_DI_ROBUST),
+  make_entry<plugins::AutorallyNNDynamics, plugins::ARRobustCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_ROBUST),
   make_entry<plugins::RacerLSTMDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_LSTM, MPPIB_COST_RACER_QUADRATIC),
   make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorQuadraticCost>(MPPIB_DYN_QUADROTOR,
                                                                           MPPIB_COST_QUADROTOR_QUADRATIC),
@@ -121,7 +124,16 @@ static const PairEntry kPairsMma[] = {
   make_entry<plugins::AutorallyNNMmaDynamics<32>, plugins::ARStandardCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_STANDARD),
   make_entry<plugins::AutorallyNNMmaDynamics<16>, plugins::ARStandardCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_STANDARD),
   make_entry<plugins::AutorallyNNMmaDynamics<8>, plugins::ARStandardCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_STANDARD),
+  make_entry<plugins::AutorallyNNMmaDynamics<32>, plugins::ARRobustCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_ROBUST),
+  make_entry<plugins::AutorallyNNMmaDynamics<16>, plugins::ARRobustCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_ROBUST),
+  make_entry<plugins::AutorallyNNMmaDynamics<8>, plugins::ARRobustCost>(MPPIB_DYN_AUTORALLY_NN, MPPIB_COST_AR_ROBUST),
 };
+
+// the costs that read a track map (MPPIB_BLOB_COSTMAP): their blobs share the mppib_ar_standard_cost_params prefix
+static bool cost_has_map(int cost_id)
+{
+  return cost_id == MPPIB_COST_AR_STANDARD || cost_id == MPPIB_COST_AR_ROBUST;
+}
 
 // pairs registered by plugin libraries (mppib_register_pair); std::vector grows, so entries are kept by pointer
 static std::vector<PairEntry*>& user_pairs()
@@ -461,7 +473,7 @@ static int check_ready(mppib_engine* e)
     return fail(MPPIB_ERR_STATE, "dynamics / cost / sampler parameter blobs must be set before solving");
   if (e->desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && !e->nn_theta_d)
     return fail(MPPIB_ERR_STATE, "MPPIB_BLOB_NN_WEIGHTS not set");
-  if (e->desc.cost_id == MPPIB_COST_AR_STANDARD && !e->costmap_tex)
+  if (cost_has_map(e->desc.cost_id) && !e->costmap_tex)
     return fail(MPPIB_ERR_STATE, "MPPIB_BLOB_COSTMAP not set");
   if (e->desc.dynamics_id == MPPIB_DYN_RACER_LSTM && !e->have_lstm)
     return fail(MPPIB_ERR_STATE, "MPPIB_BLOB_LSTM_WEIGHTS not set");
@@ -657,6 +669,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (!entry)
     return fail(MPPIB_ERR_UNSUPPORTED, "no kernel registered for dynamics %d + cost %d", desc->dynamics_id,
                 desc->cost_id);
+  // the wgmma kernel (rollout_kernel_nn_tc.cuh) is built for ARStandardCost only: refuse rather than run another kernel
+  if (desc->dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc->cost_id == MPPIB_COST_AR_ROBUST &&
+      ((desc->flags & MPPIB_FLAG_NN_TENSOR) || getenv("MPPIB_NN_TENSOR")))
+    return fail(MPPIB_ERR_UNSUPPORTED, "MPPIB_FLAG_NN_TENSOR: the tensor-core Autorally kernel supports ARStandardCost only, "
+                                       "not ARRobustCost");
 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
@@ -1361,7 +1378,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
     }
     case MPPIB_BLOB_COSTMAP:
     {
-      if (e->desc.cost_id != MPPIB_COST_AR_STANDARD)
+      if (!cost_has_map(e->desc.cost_id))
         return fail(MPPIB_ERR_INVALID_ARG, "costmap given to a cost without a map");
       if (!e->have_cost)
         return fail(MPPIB_ERR_STATE, "set MPPIB_BLOB_COST_PARAMS (map_width/map_height) before the costmap");

@@ -329,14 +329,16 @@ struct Pair
   }
   static constexpr bool kHasTensorCoreVariant = std::is_same<DYN, plugins::AutorallyNNDynamics>::value &&
                                                 std::is_same<COST, plugins::ARStandardCost>::value;
+  // the warp-specialised K1 runs either map cost (rollout_kernel_ar_ws.cuh is templated on it)
   static constexpr bool kHasWarpSpecVariant = std::is_same<DYN, plugins::AutorallyNNMmaDynamics<32>>::value &&
-                                              std::is_same<COST, plugins::ARStandardCost>::value;
+                                              (std::is_same<COST, plugins::ARStandardCost>::value ||
+                                               std::is_same<COST, plugins::ARRobustCost>::value);
   // the warp-specialised K1 the engine runs (samples per producer warp, write-back, streaming form)
-  static ArWsKernel ar_ws_kernel(const mppib_engine& e)
+  static ArWsKernel<COST> ar_ws_kernel(const mppib_engine& e)
   {
     const bool wb = e.writeback, st = e.stream_k1;
-    return e.ws_pspw == 16 ? ar_ws_kernel_for<16>(wb, st)
-                           : (e.ws_pspw == 8 ? ar_ws_kernel_for<8>(wb, st) : ar_ws_kernel_for<32>(wb, st));
+    return e.ws_pspw == 16 ? ar_ws_kernel_for<COST, 16>(wb, st)
+                           : (e.ws_pspw == 8 ? ar_ws_kernel_for<COST, 8>(wb, st) : ar_ws_kernel_for<COST, 32>(wb, st));
   }
   static int prepare(mppib_engine& e)
   {

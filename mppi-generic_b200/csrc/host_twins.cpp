@@ -573,9 +573,144 @@ static int output_trajectory_impl(const void* dyn_params, const FnnT* nn, const 
   return MPPIB_OK;
 }
 
+// ---- robust costs (host bodies) ----------------------------------------------------------------------------------------
+// utils/math_utils.h:90-94,149-155
+static inline float lin_interp(const float x, const float x_min, const float x_max, const float y_min, const float y_max)
+{
+  return (x - x_min) / (x_max - x_min) * (y_max - y_min) + y_min;
+}
+static inline float norm_dist_from_center(const float r, const float r_in, const float r_out)
+{
+  float r_center = (r_in + r_out) / 2.0f;
+  float r_width = (r_out - r_in);
+  float dist_from_center = fabsf(r - r_center);
+  return dist_from_center / (r_width * 0.5f);
+}
+// double_integrator_robust_cost.cu:41-69 — the HOST body: steep boundary 0.75 and steep cost 0.1 * crash_cost (the device
+// body, csrc/plugins/costs.cuh, uses 0.5 and 0.5 * crash_cost)
+float di_robust_state_cost(const mppib_di_circle_cost_params& p, const float* s)
+{
+  float radial_position = s[0] * s[0] + s[1] * s[1];
+  float current_velocity = sqrtf(s[2] * s[2] + s[3] * s[3]);
+  float current_angular_momentum = s[0] * s[3] - s[1] * s[2];
+  float cost = 0;
+  float normalized_dist_from_center =
+      norm_dist_from_center(std::sqrt(radial_position), std::sqrt(p.inner_path_radius2), std::sqrt(p.outer_path_radius2));
+  float steep_percent_boundary = 0.75;
+  float steep_cost = 0.1 * p.crash_cost;  // double product, narrowed
+  if (normalized_dist_from_center <= steep_percent_boundary)
+    cost += lin_interp(normalized_dist_from_center, 0, steep_percent_boundary, 0, steep_cost);
+  else if (normalized_dist_from_center > steep_percent_boundary && normalized_dist_from_center <= 1.0)
+    cost += lin_interp(normalized_dist_from_center, steep_percent_boundary, 1, steep_cost, p.crash_cost);
+  else
+    cost += p.crash_cost;
+  cost += p.velocity_cost * powf(current_velocity - p.velocity_desired, 2);
+  cost += p.velocity_cost * powf(current_angular_momentum - p.angular_momentum_desired, 2);
+  return cost;
+}
+// ar_robust_cost.cu:13-38 (host and device share this body)
+float ar_robust_stabilizing_cost(const mppib_ar_robust_cost_params& p, const float* s)
+{
+  float penalty_val = 0;
+  float slip;
+  if (std::fabs(s[4]) < 0.001)
+    slip = 0;
+  else
+    slip = std::fabs(-std::atan(s[5] / std::fabs(s[4])));
+  if (slip >= 0.75 * p.max_slip_ang)
+  {
+    float slip_val = fminf(1.0, slip / p.max_slip_ang);
+    float alpha = (slip_val - 0.75) / (1.0 - 0.75);
+    penalty_val = alpha * p.crash_coeff;
+  }
+  if (std::fabs(s[3]) >= M_PI_2)
+    penalty_val = p.crash_coeff;
+  return p.slip_coeff * slip + penalty_val;
+}
+// ar_robust_cost.cu:40-117, host branch: cosf / sinf, nearest texel by std::round after the clamps of :64-70
+float ar_robust_costmap_cost(const mppib_ar_robust_cost_params& p, const float* track_costs, const float* s)
+{
+  float cost = 0;
+  float x_front = s[0] + p.front_d * cosf(s[2]);
+  float y_front = s[1] + p.front_d * sinf(s[2]);
+  float x_back = s[0] + p.back_d * cosf(s[2]);
+  float y_back = s[1] + p.back_d * sinf(s[2]);
+  auto texel = [&](float x, float y) {
+    float u = p.r_c1[0] * x + p.r_c2[0] * y + p.trs[0];
+    float v = p.r_c1[1] * x + p.r_c2[1] * y + p.trs[1];
+    float w = p.r_c1[2] * x + p.r_c2[2] * y + p.trs[2];
+    float qx = u / w * p.map_width - 0.5f;
+    float qy = v / w * p.map_height - 0.5f;
+    qx = fmaxf(0.0f, fminf(p.map_width - 1, qx));
+    qy = fmaxf(0.0f, fminf(p.map_height - 1, qy));
+    return track_costs + 4 * ((size_t)std::round(qy) * p.map_width + (size_t)std::round(qx));
+  };
+  const float* front = texel(x_front, y_front);
+  const float* back = texel(x_back, y_back);
+  float constraint_val = fminf(1.0, fmaxf(front[0], back[0]));
+  if (constraint_val >= p.boundary_threshold)
+  {
+    float alpha = (constraint_val - p.boundary_threshold) / (1.0 - p.boundary_threshold);
+    cost += alpha * p.crash_coeff;
+  }
+  if (front[1] > p.track_slop)
+    cost += p.track_coeff * front[1];
+  if (p.desired_speed == -1)
+    cost += p.speed_coeff * std::fabs(s[4] - front[2]);
+  else
+    cost += p.speed_coeff * std::fabs(s[4] - p.desired_speed);
+  cost += p.heading_coeff * std::fabs(sinf(s[2]) + front[3]);
+  return cost;
+}
+
 }  // namespace
 
 extern "C" {
+
+int mppib_host_state_cost(int cost_id, const void* params, const float* costmap, const float* y, int t, int* crash,
+                          float* cost)
+{
+  (void)t;
+  (void)crash;  // neither robust cost reads the time step or the crash flag
+  if (!params || !y || !cost)
+    return MPPIB_ERR_INVALID_ARG;
+  switch (cost_id)
+  {
+    case MPPIB_COST_DI_ROBUST:
+      *cost = di_robust_state_cost(*static_cast<const mppib_di_circle_cost_params*>(params), y);
+      return MPPIB_OK;
+    case MPPIB_COST_AR_ROBUST:
+    {
+      const auto& p = *static_cast<const mppib_ar_robust_cost_params*>(params);
+      if (!costmap || p.map_width <= 0 || p.map_height <= 0)
+        return MPPIB_ERR_INVALID_ARG;
+      float c = ar_robust_stabilizing_cost(p, y) + ar_robust_costmap_cost(p, costmap, y);  // ar_robust_cost.cu:119-132
+      if (c > 1e16f || std::isnan(c))
+        c = 1e16f;  // MAX_COST_VALUE
+      *cost = c;
+      return MPPIB_OK;
+    }
+    default:
+      return MPPIB_ERR_UNSUPPORTED;
+  }
+}
+
+int mppib_host_ar_robust_stabilizing_cost(const mppib_ar_robust_cost_params* params, const float* s, float* cost)
+{
+  if (!params || !s || !cost)
+    return MPPIB_ERR_INVALID_ARG;
+  *cost = ar_robust_stabilizing_cost(*params, s);
+  return MPPIB_OK;
+}
+
+int mppib_host_ar_robust_costmap_cost(const mppib_ar_robust_cost_params* params, const float* costmap, const float* s,
+                                      float* cost)
+{
+  if (!params || !costmap || !s || !cost || params->map_width <= 0 || params->map_height <= 0)
+    return MPPIB_ERR_INVALID_ARG;
+  *cost = ar_robust_costmap_cost(*params, costmap, s);
+  return MPPIB_OK;
+}
 
 int mppib_host_dims(int dyn_id, int* S, int* C, int* O)
 {

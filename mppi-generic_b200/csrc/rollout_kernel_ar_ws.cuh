@@ -1,5 +1,6 @@
 /*
  * rollout_kernel_ar_ws.cuh — K1 for the Autorally pair (NeuralNetModel<7,2,3> + ARStandardCost), warp-specialised.
+ * Templated on the map cost: ARRobustCost (ar_robust_cost.cu:13-132) runs in the consumers the same way.
  *
  * Same contract as rollout_kernel<AutorallyNNMmaDynamics<32>, ARStandardCost, 1, WB, 1> (rollout_kernel.cuh): one pass over
  * the noise, per-sample cost, block partials of the softmin-weighted control average; the reference functions it replaces are
@@ -81,14 +82,17 @@ constexpr int kNoiseRing = 3;
 }  // namespace ar_ws
 
 using ArWsDyn = plugins::AutorallyNNMmaDynamics<32>;
-using ArWsArgs = RolloutArgs<ArWsDyn, plugins::ARStandardCost>;
+// the kernel's parameter block for map cost COST (ARStandardCost or ARRobustCost)
+template <class COST>
+using ArWsArgs = RolloutArgs<ArWsDyn, COST>;
 
 namespace ar_ws
 {
 // the constrained controls of one 16-byte noise group (steps t0 and t0 + 1) of one sample, as the generic kernel forms them
 // (sample_control + enforceConstraints: gaussian.cu:101-121, dynamics.cu:97-116); the second step's pair is unused when
 // t0 + 1 == T
-__device__ __forceinline__ float2 step_controls(const ArWsArgs& args, const float* means_s, float2 e, int t, bool zn, bool pn)
+template <class ARGS>
+__device__ __forceinline__ float2 step_controls(const ARGS& args, const float* means_s, float2 e, int t, bool zn, bool pn)
 {
   const float2 m = *reinterpret_cast<const float2*>(means_s + 2 * t);
   const bool um = zn || t < args.opt_stride;
@@ -97,7 +101,8 @@ __device__ __forceinline__ float2 step_controls(const ArWsArgs& args, const floa
   ArWsDyn::enforceConstraints(args.dyn, nullptr, u);
   return make_float2(u[0], u[1]);
 }
-__device__ __forceinline__ float4 group_controls(const ArWsArgs& args, const float* means_s, float4 e, int t0, bool zn,
+template <class ARGS>
+__device__ __forceinline__ float4 group_controls(const ARGS& args, const float* means_s, float4 e, int t0, bool zn,
                                                  bool pn)
 {
   const float2 u = step_controls(args, means_s, make_float2(e.x, e.y), t0, zn, pn);
@@ -115,9 +120,9 @@ __device__ __forceinline__ float4 group_controls(const ArWsArgs& args, const flo
 // with slab k + 1. The consumers turn their rows' groups into constrained controls in place, kRing groups ahead, with the
 // same operations as phase 0 (controls_in_place below), and the epilogue recomputes them from a second read of eps
 // (rollout_kernel.cuh, STREAM).
-template <bool WRITEBACK, int PSPW, bool STREAM>
+template <class COST, bool WRITEBACK, int PSPW, bool STREAM>
 __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
-    rollout_kernel_ar_ws(const __grid_constant__ ArWsArgs args, const __grid_constant__ CUtensorMap tmap)
+    rollout_kernel_ar_ws(const __grid_constant__ ArWsArgs<COST> args, const __grid_constant__ CUtensorMap tmap)
 {
   static_assert(PSPW == 32 || PSPW == 16 || PSPW == 8, "samples per producer warp");
   static_assert(ar_ws::kNoiseRing >= 3, "the refill of slab k + 1 waits for slab k - 2");
@@ -127,7 +132,6 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
   constexpr bool BOT = PSPW >= 16;              // rows g + 8 of the tile carry samples
   constexpr int NR = PSPW / 8;                  // rows a producer lane carries (g + 8 j)
   using DYN = ArWsDyn;
-  using COST = plugins::ARStandardCost;
   constexpr int S = 7, C = 2, O = 8;
   using namespace ar_ws;
 
@@ -568,14 +572,15 @@ __global__ void __launch_bounds__(ar_ws::maxThreads(PSPW), 1)
   }
 }
 
-// the instantiation for PSPW samples per producer warp, control write-back and the streaming form
-using ArWsKernel = void (*)(ArWsArgs, CUtensorMap);
-template <int PSPW>
-inline ArWsKernel ar_ws_kernel_for(bool writeback, bool stream)
+// the instantiation for map cost COST, PSPW samples per producer warp, control write-back and the streaming form
+template <class COST>
+using ArWsKernel = void (*)(ArWsArgs<COST>, CUtensorMap);
+template <class COST, int PSPW>
+inline ArWsKernel<COST> ar_ws_kernel_for(bool writeback, bool stream)
 {
   if (stream)
-    return writeback ? rollout_kernel_ar_ws<true, PSPW, true> : rollout_kernel_ar_ws<false, PSPW, true>;
-  return writeback ? rollout_kernel_ar_ws<true, PSPW, false> : rollout_kernel_ar_ws<false, PSPW, false>;
+    return writeback ? rollout_kernel_ar_ws<COST, true, PSPW, true> : rollout_kernel_ar_ws<COST, false, PSPW, true>;
+  return writeback ? rollout_kernel_ar_ws<COST, true, PSPW, false> : rollout_kernel_ar_ws<COST, false, PSPW, false>;
 }
 
 }  // namespace mppib

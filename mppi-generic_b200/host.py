@@ -27,6 +27,7 @@ FLT_MAX = 3.4028234663852886e38
 # plugin ids (include/mppi_b200/params.h)
 DYN_CARTPOLE, DYN_DOUBLE_INTEGRATOR, DYN_AUTORALLY_NN, DYN_RACER_LSTM, DYN_QUADROTOR = 0, 1, 2, 3, 4
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
+COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
 SAMPLER_GAUSSIAN, SAMPLER_COLORED_NOISE, SAMPLER_NLN = 0, 1, 2
 BLOB_DYN, BLOB_COST, BLOB_SAMPLER, BLOB_NN_WEIGHTS, BLOB_COSTMAP, BLOB_LSTM_WEIGHTS, BLOB_ELEVATION_MAP = range(7)
 FLAG_WRITEBACK_CONTROLS, FLAG_NO_TMA, FLAG_CURAND_HOST_API, FLAG_NO_PREFETCH, FLAG_NN_TENSOR, FLAG_RMPPI = 1, 2, 4, 8, 16, 32
@@ -230,6 +231,11 @@ class ARStandardCostParams(C.Structure):
                 ("back_d", C.c_float), ("map_width", C.c_int), ("map_height", C.c_int)]
 
 
+class ARRobustCostParams(C.Structure):
+    """mppib_ar_robust_cost_params: the ARStandardCostParams fields in the same order, then heading_coeff."""
+    _fields_ = ARStandardCostParams._fields_ + [("heading_coeff", C.c_float)]
+
+
 class GaussianParams(C.Structure):
     _fields_ = [("std_dev", C.c_float * (MAX_C * MAX_D)), ("control_cost_coeff", C.c_float * MAX_C),
                 ("pure_noise_trajectories_percentage", C.c_float), ("std_dev_decay", C.c_float),
@@ -268,6 +274,7 @@ ABI_SYMBOLS = [
     "mppib_host_elevation_at_world_pose", "mppib_host_static_settling", "mppib_host_lstm_initialize",
     "mppib_set_rmppi", "mppib_init_eval", "mppib_set_tsallis", "mppib_sample_trajectories", "mppib_nominal_trajectory", "mppib_compute_control", "mppib_host_npz_read", "mppib_comm_p2p_handle", "mppib_comm_p2p_open", "mppib_host_rmppi_line_search_weights", "mppib_host_rmppi_candidates",
     "mppib_host_rmppi_best_index", "mppib_set_ddp", "mppib_ddp_feedback",
+    "mppib_host_state_cost", "mppib_host_ar_robust_stabilizing_cost", "mppib_host_ar_robust_costmap_cost",
 ]
 
 _lib = None
@@ -314,6 +321,9 @@ def lib() -> C.CDLL:
     L.mppib_last_error.restype = C.c_char_p
     L.mppib_host_dims.argtypes = [C.c_int, ip, ip, ip]
     L.mppib_host_enforce_constraints.argtypes = [C.c_int, vp, vp]
+    L.mppib_host_state_cost.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp]
+    L.mppib_host_ar_robust_stabilizing_cost.argtypes = [vp, vp, vp]
+    L.mppib_host_ar_robust_costmap_cost.argtypes = [vp, vp, vp, vp]
     L.mppib_host_step.argtypes = [C.c_int, vp, vp, vp, vp, C.c_float, vp, vp, vp]
     L.mppib_host_smooth_controls.argtypes = [vp, vp, C.c_int, C.c_int]
     L.mppib_host_smooth_controls.restype = None
@@ -921,6 +931,16 @@ class ARStandardCost(_Cost):
         self.setCostmap(tex, w, h)
         return tex
 
+    def setTrackTransform(self, x_min: float, x_max: float, y_min: float, y_max: float) -> None:
+        """The world->texture transform of ARStandardCostImpl::loadTrackData (ar_standard_cost.cu:416-474):
+        R = diag(1/(x_max-x_min), 1/(y_max-y_min), 1), trs = (-x_min/(x_max-x_min), -y_min/(y_max-y_min), 1)."""
+        R = np.zeros((3, 3), np.float32)
+        R[0, 0] = 1.0 / (x_max - x_min)
+        R[1, 1] = 1.0 / (y_max - y_min)
+        R[2, 2] = 1.0
+        trs = [-x_min / (x_max - x_min), -y_min / (y_max - y_min), 1.0]
+        self.updateTransform(R, trs)
+
     def loadTrackData(self, channel0: np.ndarray, x_min: float, x_max: float, y_min: float, y_max: float,
                       ppm: float) -> None:
         """In-memory equivalent of ARStandardCostImpl::loadTrackData (ar_standard_cost.cu:416-474) for a map given as
@@ -930,12 +950,84 @@ class ARStandardCost(_Cost):
         tex = np.zeros((h, w, 4), np.float32)
         tex[..., 0] = channel0
         self.setCostmap(tex, w, h)
-        R = np.zeros((3, 3), np.float32)
-        R[0, 0] = 1.0 / (x_max - x_min)
-        R[1, 1] = 1.0 / (y_max - y_min)
-        R[2, 2] = 1.0
-        trs = [-x_min / (x_max - x_min), -y_min / (y_max - y_min), 1.0]
-        self.updateTransform(R, trs)
+        self.setTrackTransform(x_min, x_max, y_min, y_max)
+
+
+def _host_state_cost(cost, y, t: int = 0, crash: int = 0) -> float:
+    """mppib_host_state_cost (host_twins.h) for one output vector."""
+    L = lib()
+    out = C.c_float()
+    cr = C.c_int(crash)
+    y = _f32(y)
+    m = None if cost.costmap is None else _f32(cost.costmap)
+    _check(L.mppib_host_state_cost(cost.COST_ID, C.byref(cost.params), None if m is None else _ptr(m), _ptr(y), int(t),
+                                   C.byref(cr), C.byref(out)))
+    return out.value
+
+
+class DoubleIntegratorRobustCost(DoubleIntegratorCircleCost):
+    """cost_functions/double_integrator/double_integrator_robust_cost.cuh: DoubleIntegratorCircleCostParams (defaults of
+    double_integrator_circle_cost.cuh:8-23). Rollouts use the reference's device body; computeStateCost is its host body,
+    whose steep-band constants differ (0.75 / 0.1 * crash_cost against 0.5 / 0.5 * crash_cost, DESIGN.md §8)."""
+    COST_ID = COST_DI_ROBUST
+
+    def computeStateCost(self, y, t: int = 0, crash_status=None) -> float:
+        return _host_state_cost(self, y, t)
+
+    def terminalCost(self, y) -> float:
+        return 0.0
+
+    def getLipshitzConstantCost(self) -> float:
+        return float(self.params.crash_cost)  # double_integrator_robust_cost.cuh:19-22
+
+
+class ARRobustCost(ARStandardCost):
+    """cost_functions/autorally/ar_robust_cost.cuh (defaults of :11-28 reproduced); map handling as ARStandardCost. The
+    costmap's four channels are all read: .x boundary, .y track position, .z speed (desired_speed == -1), .w heading."""
+    COST_ID = COST_AR_ROBUST
+
+    def __init__(self):
+        super().__init__()
+        std = self.params
+        p = ARRobustCostParams()
+        for name, _ in ARStandardCostParams._fields_:
+            setattr(p, name, getattr(std, name))
+        p.control_cost_coeff[0] = p.control_cost_coeff[1] = 0.0
+        p.desired_speed, p.max_slip_ang = -1.0, 1.5
+        p.track_coeff, p.slip_coeff, p.speed_coeff = 33.0, 0.0, 20.0
+        p.crash_coeff, p.boundary_threshold, p.track_slop = 125000.0, 0.75, 0.0
+        p.heading_coeff = 0.0
+        self.params = p
+
+    def setTrackData(self, texels_float4: np.ndarray, x_min: float, x_max: float, y_min: float, y_max: float) -> None:
+        """A four-channel map [height][width][4] and its world bounds."""
+        t = _f32(texels_float4)
+        self.setCostmap(t, t.shape[1], t.shape[0])
+        self.setTrackTransform(x_min, x_max, y_min, y_max)
+
+    def getStabilizingCost(self, s) -> float:
+        """ar_robust_cost.cu:13-38."""
+        out = C.c_float()
+        _check(lib().mppib_host_ar_robust_stabilizing_cost(C.byref(self.params), _ptr(_f32(s)), C.byref(out)))
+        return out.value
+
+    def getCostmapCost(self, s) -> float:
+        """ar_robust_cost.cu:40-117, host branch (nearest texel)."""
+        if self.costmap is None:
+            raise MppibError(-9, "ARRobustCost has no costmap (call loadTrackData / setTrackData)")
+        out = C.c_float()
+        m = _f32(self.costmap)
+        _check(lib().mppib_host_ar_robust_costmap_cost(C.byref(self.params), _ptr(m), _ptr(_f32(s)), C.byref(out)))
+        return out.value
+
+    def computeStateCost(self, y, t: int = 0, crash_status=None) -> float:
+        """ar_robust_cost.cu:119-139."""
+        if self.costmap is None:
+            raise MppibError(-9, "ARRobustCost has no costmap (call loadTrackData / setTrackData)")
+        return _host_state_cost(self, y, t)
+
+    def terminalCost(self, y) -> float:
+        return 0.0
 
 
 class QuadrotorQuadraticCost(_Cost):
@@ -1075,9 +1167,9 @@ class Engine:
             m = self.dyn.tex_helper_.blob()
             if m is not None:  # TwoDTextureHelper::copyToDevice
                 _check(L.mppib_set_blob(self._h, BLOB_ELEVATION_MAP, m.ctypes.data, m.nbytes))
-        if self.cost.COST_ID == COST_AR_STANDARD:
+        if self.cost.COST_ID in (COST_AR_STANDARD, COST_AR_ROBUST):
             if self.cost.costmap is None:
-                raise MppibError(-9, "ARStandardCost has no costmap (call loadTrackData / setCostmap)")
+                raise MppibError(-9, f"{type(self.cost).__name__} has no costmap (call loadTrackData / setCostmap)")
             m = _f32(self.cost.costmap)
             _check(L.mppib_set_blob(self._h, BLOB_COSTMAP, _ptr(m), m.nbytes))
 

@@ -124,6 +124,47 @@ def autorally(N: int = 32768, T: int = 100) -> Workload:
     return Workload(f"autorally_nn_N{N}_T{T}", "vanilla", dyn, cost, sampler, N, T, 1, 0.02, 6.67, 0.0, x0, U0)
 
 
+def track_map_robust() -> tuple:
+    """In-memory replica of `track_map_robust.npz` (scripts/autorally/test/generateTestMaps.py:76-109): width 70, height 55
+    at 20 ppm, bounds x in [-25, 45], y in [-50, 5]. The script fills [1400][1100] arrays (i: y = i/ppm, j: x = j/ppm)
+    with channel0 = 1 where x > 50 or x < 15, else 0.6 where x > 40 or x < 25, else 0; channel1 = |55/2 - y| + x/70;
+    channel2 = x; channel3 = atan2(y, x), and stores them flattened; ARStandardCostImpl::loadTrackData reads each flat
+    channel as [height 1100][width 1400] rows. Returns (texels [1100][1400][4], x bounds, y bounds, ppm)."""
+    ppm, width, height = 20, 70, 55
+    i = np.arange(width * ppm, dtype=np.float64)[:, None]
+    j = np.arange(height * ppm, dtype=np.float64)[None, :]
+    x, y = j / ppm + 0.0 * i, i / ppm + 0.0 * j
+    ch0 = np.where((x > 50) | (x < 15), 1.0, np.where((x > 40) | (x < 25), 0.6, 0.0))
+    ch1 = np.abs(height / 2.0 - y) + x / width
+    ch3 = np.arctan2(y, x)
+    tex = np.stack([c.astype(np.float32).reshape(-1) for c in (ch0, ch1, x, ch3)], axis=-1)
+    return tex.reshape(height * ppm, width * ppm, 4), (-25.0, 45.0), (-50.0, 5.0), float(ppm)
+
+
+def autorally_robust(N: int = 32768, T: int = 100) -> Workload:
+    """The C4 model with ARRobustCost on `track_map_robust()`: the robust cost's defaults (ar_robust_cost.cuh:11-28; speed
+    from the map's .z channel) plus heading_coeff 20 (the reference's robust-cost test fixture), so every term is live.
+    The start (22.5, 0) lies in the map's zero-boundary band."""
+    w = autorally(N, T)
+    cost = H.ARRobustCost()
+    tex, xb, yb, _ = track_map_robust()
+    cost.setTrackData(tex, xb[0], xb[1], yb[0], yb[1])
+    cost.params.heading_coeff = 20.0
+    w.cost = cost
+    w.x0[0, :2] = [22.5137, 0.0071]
+    w.name = f"autorally_robust_N{N}_T{T}"
+    return w
+
+
+def double_integrator_robust_tube(N: int = 16384, T: int = 150) -> Workload:
+    """C3 with DoubleIntegratorRobustCost (examples/double_integrator_CORL2020.cu runTubeRC: crash_cost 100)."""
+    w = double_integrator_tube(N, T)
+    w.cost = H.DoubleIntegratorRobustCost()
+    w.cost.params.crash_cost = 100.0
+    w.name = f"double_integrator_robust_tube_N{N}_T{T}"
+    return w
+
+
 def synthetic_lstm_weights(hidden_dim: int = 4, head_hidden: int = 20, seed: int = 2) -> tuple:
     """(lstm, head) ~ U(-1,1)/sqrt(fan_in) in the reference's packed layouts (lstm_helper.cu:72-88, fnn_helper.cu:176-183),
     initial hidden / cell state zero (SURVEY §8d C5). The RACER networks are not in the reference tree."""
@@ -199,6 +240,8 @@ BUILDERS = {
     "double_integrator_tube": double_integrator_tube,
     "double_integrator_vanilla": double_integrator_vanilla,
     "autorally": autorally,
+    "autorally_robust": autorally_robust,
+    "double_integrator_robust_tube": double_integrator_robust_tube,
     "quadrotor": quadrotor,
 }
 
