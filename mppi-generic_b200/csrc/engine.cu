@@ -22,7 +22,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <string>
 #include <type_traits>
 #include <mutex>
@@ -499,6 +498,259 @@ static void read_result(mppib_engine& e, float* U_out, mppib_solve_stats* stats)
   }
 }
 
+// ---- choice of the rollout kernel (K1) ----------------------------------------------------------------------------
+// The descriptor flags and environment variables that choose K1's form or geometry, for A/B runs and tests of each form.
+// Read once per mppib_create; each rule below validates the values it uses.
+struct K1Overrides
+{
+  bool no_tma;     // MPPIB_FLAG_NO_TMA / MPPIB_NO_TMA: stage the noise with plain loads, never TMA
+  bool nn_tensor;  // MPPIB_FLAG_NN_TENSOR / MPPIB_NN_TENSOR: Autorally network on wgmma (rollout_kernel_nn_tc.cuh)
+  bool nn_ffma2;   // MPPIB_FLAG_NN_FFMA2 / MPPIB_NN_FFMA2: Autorally network as FP32 FFMA2s (the round-1 form)
+  bool nn_mma;     // MPPIB_FLAG_NN_MMA: Autorally network on mma.sync even with one of the two above
+  bool lstm_simt;  // MPPIB_FLAG_LSTM_SIMT / MPPIB_LSTM_SIMT: one-thread-per-sample LSTM at hidden_dim 32
+  bool no_ws;      // MPPIB_FLAG_NO_WARP_SPEC / MPPIB_NO_WS: generic kernel for the Autorally pair
+  bool bx_set;     // MPPIB_BX: samples per CTA
+  int bx;
+  bool spw_set;    // MPPIB_SPW = 32 / 16 / 8: samples per warp of the generic Autorally kernel (set: no warp-spec)
+  int spw;
+  int spt;         // MPPIB_SPT: samples per thread (0: unset)
+  int ws_pspw;     // MPPIB_WS_PSPW = 32 / 16 / 8: samples per producer warp of the warp-specialised kernel (0: unset)
+  bool stream_set; // MPPIB_STREAM = 0 / 1: force the resident or the streaming form
+  bool stream;
+  bool stream_readback;  // MPPIB_STREAM_READBACK: generic streaming form writes its controls back and re-reads them
+};
+static K1Overrides read_k1_overrides(const mppib_desc& desc)
+{
+  const char* bx = getenv("MPPIB_BX");
+  const char* spw = getenv("MPPIB_SPW");
+  const char* spt = getenv("MPPIB_SPT");
+  const char* ws_pspw = getenv("MPPIB_WS_PSPW");
+  const char* stream = getenv("MPPIB_STREAM");
+  K1Overrides o;
+  o.no_tma = (desc.flags & MPPIB_FLAG_NO_TMA) || getenv("MPPIB_NO_TMA");
+  o.nn_tensor = (desc.flags & MPPIB_FLAG_NN_TENSOR) || getenv("MPPIB_NN_TENSOR");
+  o.nn_ffma2 = (desc.flags & MPPIB_FLAG_NN_FFMA2) || getenv("MPPIB_NN_FFMA2");
+  o.nn_mma = (desc.flags & MPPIB_FLAG_NN_MMA) != 0;
+  o.lstm_simt = (desc.flags & MPPIB_FLAG_LSTM_SIMT) || getenv("MPPIB_LSTM_SIMT");
+  o.no_ws = (desc.flags & MPPIB_FLAG_NO_WARP_SPEC) || getenv("MPPIB_NO_WS");
+  o.bx_set = bx != nullptr;
+  o.bx = bx ? atoi(bx) : 0;
+  o.spw_set = spw != nullptr;
+  o.spw = spw ? atoi(spw) : 0;
+  o.spt = spt ? atoi(spt) : 0;
+  o.ws_pspw = ws_pspw ? atoi(ws_pspw) : 0;
+  o.stream_set = stream != nullptr;
+  o.stream = stream && atoi(stream) != 0;
+  o.stream_readback = getenv("MPPIB_STREAM_READBACK") != nullptr;
+  return o;
+}
+
+// The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
+// tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
+static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairEntry** out)
+{
+  const PairEntry* entry = nullptr;
+  for (const auto& p : kPairs)
+    if (p.dyn_id == desc.dynamics_id && p.cost_id == desc.cost_id)
+      entry = &p;
+  for (const PairEntry* p : user_pairs())  // out-of-tree pairs (mppib_load_plugin / mppib_register_pair)
+    if (p->dyn_id == desc.dynamics_id && p->cost_id == desc.cost_id)
+      entry = p;
+  // Autorally pair: the network runs on register-level mma.sync by default (plugins/nn_mma.cuh). NN_FFMA2 keeps the FFMA2
+  // form, NN_TENSOR selects the wgmma kernel (which is built on the FFMA2 entry).
+  if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(ov.nn_ffma2 || ov.nn_tensor) || ov.nn_mma))
+  {
+    // samples per warp of the generic kernel's network (plugins/nn_mma.cuh): 32. Narrower sample groups (MPPIB_SPW = 16 / 8)
+    // halve / quarter a warp's tensor work per step, but the step time of a lone warp barely moves: the chain, not the
+    // work, is the limit — which the warp-specialised kernel (rollout_kernel_ar_ws.cuh, the default for D == 1) removes instead.
+    const int spw = (ov.spw == 16 || ov.spw == 8) ? ov.spw : 32;
+    for (const auto& p : kPairsMma)
+      if (p.cost_id == desc.cost_id && p.spw == spw)
+        entry = &p;
+  }
+  // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
+  // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network.
+  if (entry && desc.dynamics_id == MPPIB_DYN_RACER_LSTM && desc.model_dims[0] == lstm_mma::H &&
+      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !ov.lstm_simt)
+    for (const auto& p : kPairsLstmMma)
+      if (p.cost_id == desc.cost_id)
+        entry = &p;
+  if (!entry)
+    return fail(MPPIB_ERR_UNSUPPORTED, "no kernel registered for dynamics %d + cost %d", desc.dynamics_id, desc.cost_id);
+  // the wgmma kernel (rollout_kernel_nn_tc.cuh) is built for ARStandardCost only: refuse rather than run another kernel
+  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc.cost_id == MPPIB_COST_AR_ROBUST && ov.nn_tensor)
+    return fail(MPPIB_ERR_UNSUPPORTED, "MPPIB_FLAG_NN_TENSOR: the tensor-core Autorally kernel supports ARStandardCost only, "
+                                       "not ARRobustCost");
+  *out = entry;
+  return MPPIB_OK;
+}
+
+// K1's form and launch geometry for an engine whose pair, sizes and flags are set: the generic, SPT = 2, RMPPI, warp-
+// specialised or wgmma kernel, resident or streaming, and bx, threads, grid, shared memory. Pair<>::kernel maps the choice
+// to the instantiation.
+static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides& ov)
+{
+  // One thread per sample; bx samples per CTA, whole-horizon noise tile resident in shared memory. The rollout is bound by
+  // the T-step dependency chain, so a CTA takes the same time whatever its width: the block width is chosen to put every CTA
+  // in ONE wave (no tail wave running at a fraction of the chip), preferring the narrowest such width (more SMs busy, fewer
+  // warps contending per scheduler); 64 if several waves are unavoidable.
+  const mppib_desc& desc = e->desc;
+  int max_smem = 0, num_sms = 0, smem_per_sm = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, desc.device));
+  CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, desc.device));
+  CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, desc.device));
+  e->num_sms = num_sms;
+  const bool tma_ok = !ov.no_tma && e->TC % 4 == 0;
+  // samples per thread (rollout_kernel.cuh): 1. SPT = 2 halves the shared-memory wavefronts per sample of the NN model
+  // but a lone warp per scheduler cannot overlap its own FFMA2 / MUFU / latency phases the
+  // way two warps do, and it measured slower. Kept selectable for experiments through MPPIB_SPT.
+  e->spt = (ov.spt >= 1 && ov.spt <= entry->max_spt && (ov.spt == 1 || e->D == 1)) ? ov.spt : 1;
+  e->lps = 32 / entry->spw;
+  const int spt = e->spt, lps = e->lps;
+  // Autorally pair, one system: the warp-specialised K1 (rollout_kernel_ar_ws.cuh) — a producer and a consumer warp per 32
+  // samples. MPPIB_NO_WS / MPPIB_SPW / MPPIB_SPT keep the generic kernel (A/B runs, tests of the generic form).
+  const bool is_mma = entry >= kPairsMma && entry < kPairsMma + sizeof(kPairsMma) / sizeof(kPairsMma[0]);
+  e->ar_ws = is_mma && entry->spw == 32 && e->D == 1 && !e->rmppi && spt == 1 && !ov.no_ws && !ov.spw_set;
+  const bool ws = e->ar_ws;
+  // samples per producer warp: 16 while the GPU is throughput-bound; 8 (four producers per 32 samples, one per scheduler)
+  // once it holds so few rollouts that a group's step time sets K1 (kWsPspw8MaxRollouts)
+  e->ws_pspw = (ov.ws_pspw == 32 || ov.ws_pspw == 16 || ov.ws_pspw == 8) ? ov.ws_pspw
+                                                                        : (e->n_local <= kWsPspw8MaxRollouts ? 8 : 16);
+  const int ws_wpg = ar_ws::warpsPerGroup(e->ws_pspw);
+  // shared memory of a CTA of b samples whose noise tile holds `chunks` 32-column slabs (all: resident; a ring: streaming)
+  auto layout = [&](int b, int chunks) {
+    const int dyn_floats = ws ? ar_ws::sharedFloats(b) : e->dyn_shared_floats_fn(desc.model_dims, b);
+    return (int)rollout_smem_layout(b, chunks, e->D, e->TC, dyn_floats, e->cost_shared_floats(e->T)).total;
+  };
+  auto smem_for = [&](int b) { return layout(b, e->nchunks); };
+  const int unit = ws ? 32 : entry->spw * spt;  // samples per warp of threads
+  const int max_bx = ws ? 32 * ar_ws::maxGroups(e->ws_pspw) : entry->max_block_threads / 32 * unit;  // samples per CTA (__launch_bounds__)
+  auto threads_for = [&](int b) { return ws ? ws_wpg * b : b / spt * lps; };
+  // resident CTAs per SM: shared memory (+1 KB the hardware reserves per CTA), threads, and for the warp-specialised kernel
+  // its 128-register budget
+  auto ctas_per_sm = [&](int b, int sm) {
+    int n = std::min(std::min(smem_per_sm / (sm + 1024), 2048 / threads_for(b)), 32);
+    if (ws)  // registers: __launch_bounds__(maxThreads, 1) lets ptxas use 65536 / maxThreads per thread
+      n = std::min(n, ar_ws::maxThreads(e->ws_pspw) / threads_for(b));
+    return n;
+  };
+  auto waves = [&](int b, int per_sm) {  // waves of CTAs of b samples at per_sm CTAs per SM
+    const long per_wave = (long)per_sm * num_sms;
+    return ((e->n_local + b - 1) / b + per_wave - 1) / per_wave;
+  };
+  int bx = ov.bx;  // MPPIB_BX, up to 512 here and clamped to max_bx below
+  if (bx < unit || bx > 512 || (bx % unit) != 0)
+    bx = 0;
+  int ws_one_wave = 0;  // warp-specialised kernel: the one-CTA-per-SM width, when __launch_bounds__ allows it
+  if (bx == 0 && ws)
+  {
+    // warp-specialised kernel: up to one warp per scheduler, one pair per CTA (no two producers ever share a scheduler);
+    // beyond that ONE CTA per SM, as narrow as covers n_local, so that every SM is busy and the kernel's alternating role
+    // table (P C C P C P P C) balances producers over the four schedulers. Wider than the resident tile fits: the wave rule
+    // below, and then the streaming form at this width.
+    const long pairs_total = (e->n_local + 31) / 32;
+    if (ws_wpg * pairs_total <= 4L * num_sms)
+      bx = 32;
+    else
+    {
+      const int need = (int)(((e->n_local + num_sms - 1) / num_sms + 31) / 32) * 32;
+      if (need <= max_bx)
+        ws_one_wave = need;
+      if (need <= max_bx && smem_for(need) <= max_smem)
+        bx = need;
+    }
+  }
+  if (bx == 0)
+  {
+    int best = 0;
+    long best_waves = 1L << 40;
+    for (int cand = ws ? unit : std::max(unit, 64 / lps); cand <= max_bx; cand += unit)
+    {
+      const int sm = smem_for(cand);
+      if (sm > max_smem)
+        break;
+      const int per_sm = ctas_per_sm(cand, sm);
+      if (per_sm < 1)
+        break;
+      const long w = waves(cand, per_sm);
+      if (w < best_waves)
+      {
+        best_waves = w;
+        best = cand;
+      }
+    }
+    bx = best ? best : unit;
+  }
+  if (bx > max_bx)
+    bx = max_bx;
+  bx = (bx / unit) * unit;  // whole warps of threads
+  if (bx < unit)
+    bx = unit;
+  while (smem_for(bx) > max_smem && bx > unit)
+    bx -= unit;
+  e->smem_bytes = (uint32_t)smem_for(bx);
+  if ((int)e->smem_bytes > max_smem)
+    return fail(MPPIB_ERR_SMEM, "noise tile needs %u B of shared memory, device allows %d", e->smem_bytes, max_smem);
+  // tensor-core variant of the Autorally pair: fixed 128-sample CTAs (one warpgroup, two m64 wgmma tiles), streaming
+  // noise ring. Opt-in: three exposed MMA round trips per step with few warps per SM to cover them
+  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc.cost_id == MPPIB_COST_AR_STANDARD && e->D == 1 && tma_ok &&
+      ov.nn_tensor)
+  {
+    e->nn_tc = true;
+    bx = nn_tc::kRows;
+    e->smem_bytes = nn_tc::layout(e->TC, e->T).total;
+    if ((int)e->smem_bytes > max_smem)
+      return fail(MPPIB_ERR_SMEM, "tensor-core rollout needs %u B of shared memory, device allows %d", e->smem_bytes,
+                  max_smem);
+  }
+  // Streaming form (STREAM in rollout_kernel.cuh and rollout_kernel_ar_ws.cuh): the noise slabs cycle through a ring, so
+  // shared memory per sample no longer grows with T. Taken when the resident tile needs several waves and the ring needs
+  // fewer; MPPIB_STREAM=0/1 overrides. The generic kernel streams through 2 buffers at 64 samples per CTA (or MPPIB_BX, here
+  // up to max_bx), only with TMA, one sample per thread, outside RMPPI and the wgmma kernel. The warp-specialised kernel
+  // streams through 3 at its one-CTA-per-SM width (on 132 SMs that is C4, N = 32768: the 256-sample resident tile does not
+  // fit, and the 96-thread CTAs the wave rule falls back to run in two waves); forced, it also runs without TMA (the issuing
+  // warp fills the ring with plain loads).
+  {
+    const int ring = ws ? ar_ws::kNoiseRing : e->ring;
+    const bool env_bx_ok = ov.bx >= unit && ov.bx <= max_bx && (ov.bx % unit) == 0;
+    const int sbx = ws ? ((ws_one_wave && !ov.bx_set) ? ws_one_wave : bx) : (env_bx_ok ? ov.bx : 64);
+    const int sm_str = layout(sbx, ring);
+    const bool auto_ok = tma_ok && e->nchunks > ring;
+    if ((ws || (auto_ok && !e->rmppi && !e->nn_tc && spt == 1)) && sm_str <= max_smem)
+    {
+      // the generic kernel asks the occupancy API (registers count too); the warp-specialised one's budget is fixed
+      const int per_sm_str = ws ? std::max(1, ctas_per_sm(sbx, sm_str))
+                                : entry->stream_blocks_per_sm(*e, threads_for(sbx), (size_t)sm_str);
+      if (per_sm_str > 0)
+      {
+        const long waves_res = waves(bx, std::max(1, ctas_per_sm(bx, smem_for(bx))));
+        bool want = auto_ok && waves_res > 1 && waves(sbx, per_sm_str) < waves_res;
+        if (ov.stream_set)
+          want = ov.stream;
+        if (want)
+        {
+          e->stream_k1 = true;
+          if (!ws && ov.stream_readback)  // A/B: the round-1 form (controls written back and re-read by the epilogue)
+            e->writeback = true;
+          bx = sbx;
+          e->smem_bytes = (uint32_t)sm_str;
+        }
+      }
+    }
+  }
+  e->bx = bx;
+  // MPPIB_FLAG_NN_MMA with NN_TENSOR keeps the mma.sync entry, which has no wgmma kernel: Pair<>::kernel runs another form
+  e->threads = (e->nn_tc && !is_mma) ? nn_tc::kRows : threads_for(bx);
+  e->dyn_shared_floats = ws ? ar_ws::sharedFloats(bx) : e->dyn_shared_floats_fn(desc.model_dims, bx);
+  e->grid = (e->n_local + bx - 1) / bx;
+  if (e->grid > kCombineMaxRecords)
+    return fail(MPPIB_ERR_UNSUPPORTED, "%d rollout blocks exceed the combine kernel's %d records; raise MPPIB_BX", e->grid,
+                kCombineMaxRecords);
+  e->use_tma = tma_ok;
+  e->stream_readback = e->stream_k1 && e->writeback && ov.stream_readback;
+  return MPPIB_OK;
+}
+
 // =================================================================================================================
 extern "C" {
 
@@ -604,6 +856,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (!out || !desc)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   *out = nullptr;
+  const K1Overrides ov = read_k1_overrides(*desc);
   if (desc->num_rollouts <= 0 || desc->num_timesteps <= 0)
     return fail(MPPIB_ERR_INVALID_ARG, "num_rollouts and num_timesteps must be positive");
   if (desc->num_distributions < 1 || desc->num_distributions > MPPIB_MAX_DISTRIBUTIONS)
@@ -632,48 +885,8 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
       return fail(MPPIB_ERR_UNSUPPORTED, "RacerDubinsElevationLSTMSteering is built for num_distributions == 1 only");
   }
   const PairEntry* entry = nullptr;
-  for (const auto& p : kPairs)
-    if (p.dyn_id == desc->dynamics_id && p.cost_id == desc->cost_id)
-      entry = &p;
-  for (const PairEntry* p : user_pairs())  // out-of-tree pairs (mppib_load_plugin / mppib_register_pair)
-    if (p->dyn_id == desc->dynamics_id && p->cost_id == desc->cost_id)
-      entry = p;
-  // Autorally pair: the network runs on register-level mma.sync by default (plugins/nn_mma.cuh). MPPIB_FLAG_NN_FFMA2 / MPPIB_NN_FFMA2 keep the FFMA2 form,
-  // MPPIB_FLAG_NN_TENSOR / MPPIB_NN_TENSOR select the wgmma kernel (which is built on the FFMA2 entry).
-  const bool nn_other = (desc->flags & (MPPIB_FLAG_NN_FFMA2 | MPPIB_FLAG_NN_TENSOR)) || getenv("MPPIB_NN_FFMA2") ||
-                        getenv("MPPIB_NN_TENSOR");
-  if (entry && desc->dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!nn_other || (desc->flags & MPPIB_FLAG_NN_MMA)))
-  {
-    // samples per warp of the generic kernel's network (plugins/nn_mma.cuh): 32. Narrower sample groups (MPPIB_SPW = 16 / 8)
-    // halve / quarter a warp's tensor work per step, but the step time of a lone warp barely moves: the chain, not the
-    // work, is the limit — which the warp-specialised kernel (rollout_kernel_ar_ws.cuh, the default for D == 1) removes instead.
-    int spw = 32;
-    if (const char* sv = getenv("MPPIB_SPW"))
-    {
-      const int v = atoi(sv);
-      if (v == 32 || v == 16 || v == 8)
-        spw = v;
-    }
-    for (const auto& p : kPairsMma)
-      if (p.cost_id == desc->cost_id && p.spw == spw)
-        entry = &p;
-  }
-  // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
-  // layout in registers (plugins/lstm_mma.cuh).
-  // MPPIB_FLAG_LSTM_SIMT / MPPIB_LSTM_SIMT keep the one-thread-per-sample network.
-  if (entry && desc->dynamics_id == MPPIB_DYN_RACER_LSTM && desc->model_dims[0] == lstm_mma::H &&
-      desc->model_dims[1] <= 8 * lstm_mma::kHeadTiles && !(desc->flags & MPPIB_FLAG_LSTM_SIMT) && !getenv("MPPIB_LSTM_SIMT"))
-    for (const auto& p : kPairsLstmMma)
-      if (p.cost_id == desc->cost_id)
-        entry = &p;
-  if (!entry)
-    return fail(MPPIB_ERR_UNSUPPORTED, "no kernel registered for dynamics %d + cost %d", desc->dynamics_id,
-                desc->cost_id);
-  // the wgmma kernel (rollout_kernel_nn_tc.cuh) is built for ARStandardCost only: refuse rather than run another kernel
-  if (desc->dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc->cost_id == MPPIB_COST_AR_ROBUST &&
-      ((desc->flags & MPPIB_FLAG_NN_TENSOR) || getenv("MPPIB_NN_TENSOR")))
-    return fail(MPPIB_ERR_UNSUPPORTED, "MPPIB_FLAG_NN_TENSOR: the tensor-core Autorally kernel supports ARStandardCost only, "
-                                       "not ARRobustCost");
+  if (int rc = pick_entry(*desc, ov, &entry))
+    return rc;
 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
@@ -736,211 +949,9 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (e->n_local <= 0)
     return bail(fail(MPPIB_ERR_INVALID_ARG, "rank %d of %d has no rollouts (N=%d)", desc->rank, world, e->N));
 
-  // launch geometry: one thread per sample; BX samples per CTA, whole-horizon noise tile resident in shared memory.
-  // The rollout is bound by the T-step dependency chain, so a CTA takes the same time whatever its width: the block
-  // width is chosen to put every CTA in ONE wave (no tail wave running at a fraction of the chip), preferring the
-  // narrowest such width (more SMs busy, fewer warps contending per scheduler); 64 if several waves are unavoidable.
-  int max_smem = 0, num_sms = 0, smem_per_sm = 0;
-  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, desc->device));
-  CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, desc->device));
-  CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, desc->device));
-  e->num_sms = num_sms;
-  std::function<int(int)> smem_for = [&](int b) {
-    return (int)rollout_smem_layout(b, e->nchunks, e->D, e->TC, e->dyn_shared_floats_fn(e->desc.model_dims, b),
-                                    e->cost_shared_floats(e->T))
-        .total;
-  };
-  // samples per thread (rollout_kernel.cuh): 1. SPT = 2 halves the shared-memory wavefronts per sample of the NN model
-  // but a lone warp per scheduler cannot overlap its own FFMA2 / MUFU / latency phases the
-  // way two warps do, and it measured slower. Kept selectable for experiments through MPPIB_SPT.
-  int spt = 1;
-  if (const char* s = getenv("MPPIB_SPT"))
-  {
-    const int v = atoi(s);
-    if (v >= 1 && v <= entry->max_spt && (v == 1 || e->D == 1))
-      spt = v;
-  }
-  e->spt = spt;
-  const int lps = 32 / entry->spw;
-  e->lps = lps;
-  // Autorally pair, one system: the warp-specialised K1 (rollout_kernel_ar_ws.cuh) — a producer and a consumer warp per 32
-  // samples. MPPIB_NO_WS / MPPIB_SPW / MPPIB_SPT keep the generic kernel (A/B runs, tests of the generic form).
-  const bool is_mma32 = entry >= kPairsMma && entry < kPairsMma + sizeof(kPairsMma) / sizeof(kPairsMma[0]) && entry->spw == 32;
-  e->ar_ws = is_mma32 && e->D == 1 && !e->rmppi && spt == 1 && !getenv("MPPIB_NO_WS") && !getenv("MPPIB_SPW") &&
-             !(desc->flags & MPPIB_FLAG_NO_WARP_SPEC);
-  const bool ws = e->ar_ws;
-  // samples per producer warp: 16 while the GPU is throughput-bound; 8 (four producers per 32 samples, one per scheduler)
-  // once it holds so few rollouts that a group's step time sets K1 (kWsPspw8MaxRollouts)
-  e->ws_pspw = e->n_local <= kWsPspw8MaxRollouts ? 8 : 16;
-  if (const char* sv = getenv("MPPIB_WS_PSPW"))
-    if (atoi(sv) == 32 || atoi(sv) == 16 || atoi(sv) == 8)
-      e->ws_pspw = atoi(sv);
-  const int ws_wpg = ar_ws::warpsPerGroup(e->ws_pspw);
-  if (ws)
-    smem_for = [&](int b) {
-      return (int)rollout_smem_layout(b, e->nchunks, 1, e->TC, ar_ws::sharedFloats(b), e->cost_shared_floats(e->T)).total;
-    };
-  const int unit = ws ? 32 : entry->spw * spt;  // samples per warp of threads
-  const int max_bx = ws ? 32 * ar_ws::maxGroups(e->ws_pspw) : entry->max_block_threads / 32 * unit;  // samples per CTA (__launch_bounds__)
-  auto threads_for = [&](int b) { return ws ? ws_wpg * b : b / spt * lps; };
-  // resident CTAs per SM: shared memory (+1 KB the hardware reserves per CTA), threads, and for the warp-specialised kernel
-  // its 128-register budget
-  auto ctas_per_sm = [&](int b, int sm) {
-    int n = std::min(std::min(smem_per_sm / (sm + 1024), 2048 / threads_for(b)), 32);
-    if (ws)  // registers: __launch_bounds__(maxThreads, 1) lets ptxas use 65536 / maxThreads per thread
-      n = std::min(n, ar_ws::maxThreads(e->ws_pspw) / threads_for(b));
-    return n;
-  };
-  int bx = 0;
-  const bool bx_set = getenv("MPPIB_BX") != nullptr;
-  if (bx_set)
-  {
-    bx = atoi(getenv("MPPIB_BX"));
-    if (bx < unit || bx > 512 || (bx % unit) != 0)
-      bx = 0;
-  }
-  int ws_one_wave = 0;  // warp-specialised kernel: the one-CTA-per-SM width, when __launch_bounds__ allows it
-  if (bx == 0 && ws)
-  {
-    // warp-specialised kernel: up to one warp per scheduler, one pair per CTA (no two producers ever share a scheduler);
-    // beyond that ONE CTA per SM, as narrow as covers n_local, so that every SM is busy and the kernel's alternating role
-    // table (P C C P C P P C) balances producers over the four schedulers. Wider than the resident tile fits: the wave rule
-    // below, and then the streaming form at this width.
-    const long pairs_total = (e->n_local + 31) / 32;
-    if (ws_wpg * pairs_total <= 4L * num_sms)
-      bx = 32;
-    else
-    {
-      const int need = (int)(((e->n_local + num_sms - 1) / num_sms + 31) / 32) * 32;
-      if (need <= max_bx)
-        ws_one_wave = need;
-      if (need <= max_bx && smem_for(need) <= max_smem)
-        bx = need;
-    }
-  }
-  if (bx == 0)
-  {
-    int best = 0;
-    long best_waves = 1L << 40;
-    for (int cand = ws ? unit : std::max(unit, 64 / lps); cand <= max_bx; cand += unit)
-    {
-      const int sm = smem_for(cand);
-      if (sm > max_smem)
-        break;
-      const int per_sm = ctas_per_sm(cand, sm);
-      if (per_sm < 1)
-        break;
-      const long blocks = (e->n_local + cand - 1) / cand;
-      const long waves = (blocks + (long)per_sm * num_sms - 1) / ((long)per_sm * num_sms);
-      if (waves < best_waves)
-      {
-        best_waves = waves;
-        best = cand;
-      }
-    }
-    bx = best ? best : unit;
-  }
-  if (bx > max_bx)
-    bx = max_bx;
-  bx = (bx / unit) * unit;  // whole warps of threads
-  if (bx < unit)
-    bx = unit;
-  while (smem_for(bx) > max_smem && bx > unit)
-    bx -= unit;
-  e->smem_bytes = (uint32_t)smem_for(bx);
-  if ((int)e->smem_bytes > max_smem)
-    return bail(fail(MPPIB_ERR_SMEM, "noise tile needs %u B of shared memory, device allows %d", e->smem_bytes,
-                     max_smem));
-  // tensor-core variant of the Autorally pair: fixed 128-sample CTAs (one warpgroup, two m64 wgmma tiles), streaming
-  // noise ring. Opt-in: three exposed MMA round trips per step with few warps per SM to cover them
-  if (desc->dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc->cost_id == MPPIB_COST_AR_STANDARD && e->D == 1 &&
-      (e->TC % 4) == 0 && !(desc->flags & MPPIB_FLAG_NO_TMA) && !getenv("MPPIB_NO_TMA") &&
-      ((desc->flags & MPPIB_FLAG_NN_TENSOR) || getenv("MPPIB_NN_TENSOR")))
-  {
-    e->nn_tc = true;
-    bx = nn_tc::kRows;
-    e->smem_bytes = nn_tc::layout(e->TC, e->T).total;
-    if ((int)e->smem_bytes > max_smem)
-      return bail(fail(MPPIB_ERR_SMEM, "tensor-core rollout needs %u B of shared memory, device allows %d",
-                       e->smem_bytes, max_smem));
-  }
-  // streaming K1 (rollout_kernel.cuh: STREAM): chosen when the resident whole-horizon tile forces several waves and the
-  // ring variant needs fewer; MPPIB_STREAM=0/1 overrides
-  {
-    const bool tma_ok = !(desc->flags & MPPIB_FLAG_NO_TMA) && (e->TC % 4 == 0) && !getenv("MPPIB_NO_TMA");
-    const int sm_res = smem_for(bx);
-    const int per_sm_res = std::max(1, ctas_per_sm(bx, sm_res));
-    const long blocks_res = (e->n_local + bx - 1) / bx;
-    const long waves_res = (blocks_res + (long)per_sm_res * num_sms - 1) / ((long)per_sm_res * num_sms);
-    int sbx = 64;
-    if (const char* sb = getenv("MPPIB_BX"))
-    {
-      const int v = atoi(sb);
-      if (v >= unit && v <= max_bx && (v % unit) == 0)
-        sbx = v;
-    }
-    const int sm_str = (int)rollout_smem_layout(sbx, e->ring, e->D, e->TC, e->dyn_shared_floats_fn(e->desc.model_dims, sbx),
-                                                e->cost_shared_floats(e->T))
-                           .total;
-    bool want = false;
-    if (tma_ok && !e->rmppi && !e->nn_tc && !ws && spt == 1 && e->nchunks > e->ring && sm_str <= max_smem)
-    {
-      const int per_sm_str = entry->stream_blocks_per_sm(e->D, threads_for(sbx), (size_t)sm_str);
-      if (per_sm_str > 0)
-      {
-        const long blocks_str = (e->n_local + sbx - 1) / sbx;
-        const long waves_str = (blocks_str + (long)per_sm_str * num_sms - 1) / ((long)per_sm_str * num_sms);
-        want = waves_res > 1 && waves_str < waves_res;
-        if (const char* sv = getenv("MPPIB_STREAM"))
-          want = atoi(sv) != 0;
-      }
-    }
-    if (want)
-    {
-      e->stream_k1 = true;
-      if (getenv("MPPIB_STREAM_READBACK"))  // A/B: the round-1 form (controls written back and re-read by the epilogue)
-        e->writeback = true;
-      bx = sbx;
-      e->smem_bytes = (uint32_t)sm_str;
-    }
-  }
-  // warp-specialised K1, streaming form (rollout_kernel_ar_ws.cuh: STREAM), by the same rule at the one-CTA-per-SM width:
-  // chosen when the resident tile needs several waves and the ring fits in fewer. On 132 SMs that is C4 (N = 32768: the
-  // 256-sample resident tile does not fit, and the 96-thread CTAs the wave rule falls back to run in two waves).
-  // MPPIB_STREAM=0/1 overrides; forced, it also runs without TMA (the issuing warp fills the ring with plain loads).
-  if (ws)
-  {
-    const bool tma_ok = !(desc->flags & MPPIB_FLAG_NO_TMA) && (e->TC % 4 == 0) && !getenv("MPPIB_NO_TMA");
-    const int sbx = (ws_one_wave && !bx_set) ? ws_one_wave : bx;
-    const int sm_str = (int)rollout_smem_layout(sbx, ar_ws::kNoiseRing, 1, e->TC, ar_ws::sharedFloats(sbx),
-                                                e->cost_shared_floats(e->T))
-                           .total;
-    if (sm_str <= max_smem)
-    {
-      auto waves = [&](int b, int sm) {
-        const long per_wave = (long)std::max(1, ctas_per_sm(b, sm)) * num_sms;
-        return ((e->n_local + b - 1) / b + per_wave - 1) / per_wave;
-      };
-      const long waves_res = waves(bx, smem_for(bx));
-      bool want = tma_ok && e->nchunks > ar_ws::kNoiseRing && waves_res > 1 && waves(sbx, sm_str) < waves_res;
-      if (const char* sv = getenv("MPPIB_STREAM"))
-        want = atoi(sv) != 0;
-      if (want)
-      {
-        e->stream_k1 = true;
-        bx = sbx;
-        e->smem_bytes = (uint32_t)sm_str;
-      }
-    }
-  }
-  e->bx = bx;
-  e->dyn_shared_floats = ws ? ar_ws::sharedFloats(bx) : e->dyn_shared_floats_fn(e->desc.model_dims, bx);
-  e->grid = (e->n_local + bx - 1) / bx;
-  if (e->grid > kCombineMaxRecords)
-    return bail(fail(MPPIB_ERR_UNSUPPORTED, "%d rollout blocks exceed the combine kernel's %d records; raise MPPIB_BX",
-                     e->grid, kCombineMaxRecords));
+  if (int rc = choose_k1(e, entry, ov))
+    return bail(rc);
   e->pstride = ((kPartialHeader + e->TC + 3) / 4) * 4;
-  e->use_tma = !(desc->flags & MPPIB_FLAG_NO_TMA) && (e->TC % 4 == 0) && !getenv("MPPIB_NO_TMA");
 
   if (desc->stream)
     e->stream = (cudaStream_t)desc->stream;
@@ -2220,7 +2231,7 @@ int mppib_get_launch_info(mppib_engine* e, int* grid, int* block, int* smem_byte
   if (grid)
     *grid = e->grid;
   if (block)
-    *block = e->nn_tc ? e->bx : (e->ar_ws ? ar_ws::warpsPerGroup(e->ws_pspw) * e->bx : e->bx / e->spt * e->lps);
+    *block = e->threads;
   if (smem_bytes)
     *smem_bytes = (int)e->smem_bytes;
   if (uses_tma)
