@@ -54,8 +54,10 @@ enum mppib_blob
   MPPIB_BLOB_NN_WEIGHTS = 3,  /* NeuralNetModel::updateModel             ar_nn_model.cu:40-45 (packed W,b per layer) */
   MPPIB_BLOB_COSTMAP = 4,     /* ARStandardCost::costmapToTexture        ar_standard_cost.cu:145-184 (float4 texels) */
   MPPIB_BLOB_LSTM_WEIGHTS = 5, /* LSTMHelper weights                     lstm_helper.cu:72-88 */
-  MPPIB_BLOB_ELEVATION_MAP = 6 /* RACER models: TwoDTextureHelper<float> map 0 (mppib_elevation_map_header + floats,
+  MPPIB_BLOB_ELEVATION_MAP = 6, /* RACER models: TwoDTextureHelper<float> map 0 (mppib_elevation_map_header + floats,
                                   params.h); optional — without it the ground is flat  racer_dubins.cu:359-434 */
+  MPPIB_BLOB_COST_TEXTURE = 7   /* QuadrotorMapCost: its tex_helper_ map 0, same format as MPPIB_BLOB_ELEVATION_MAP;
+                                   optional — without it the costmap term is 0  quadrotor_map_cost.cu:359-395 */
 };
 
 /* Flags for mppib_desc.flags */

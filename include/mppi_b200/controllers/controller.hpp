@@ -135,6 +135,7 @@ public:
   }
   virtual ~Controller()
   {  // controller.cuh:194-216: the controller frees the device side, not the plugin objects
+    bindCostEngine(cost_, nullptr);
     if (engine_)
       mppib_destroy(engine_);
   }
@@ -519,6 +520,7 @@ public:
     MPPIB_HANDLE(mppib_set_blob(engine_, MPPIB_BLOB_SAMPLER_PARAMS, &sb, sizeof(sb)));
     MPPIB_HANDLE(model_->pushModelBlobs(engine_));  // NN / LSTM weights
     pushCostmap(cost_);
+    pushCostBlobs(cost_);
     MPPIB_HANDLE(mppib_set_solver(engine_, params_.dt_, params_.lambda_, params_.alpha_));
   }
   // kept for source compatibility (controller.cuh:299-302,886-894); the engine has a single fused kernel
@@ -761,6 +763,7 @@ protected:
     model_->fillModelDims(d.model_dims);
     MPPIB_HANDLE(mppib_create(&engine_, &d));
     pushParams();
+    bindCostEngine(cost_, engine_);
     bindFeedback();
     // createAndSeedCUDARandomNumberGen (controller.cu:192-198) for a new controller; the old position for a re-creation
     MPPIB_HANDLE(mppib_seed(engine_, params_.seed_, recreated ? rng_offset : 0ULL));
@@ -774,6 +777,25 @@ protected:
       MPPIB_HANDLE(mppib_set_blob(engine_, MPPIB_BLOB_COSTMAP, c->costmap(), c->costmapBytes()));
   }
   void pushCostmap(...)
+  {
+  }
+  // costs that push more than their parameter blob (QuadrotorMapCost: tex_helper_'s map), and that push it themselves when
+  // their parameters change (updateWaypoint): they learn the engine of the controller built on them
+  template <class C>
+  auto pushCostBlobs(C* c) -> decltype(c->pushCostBlobs((mppib_engine*)nullptr), void())
+  {
+    c->pushCostBlobs(engine_);
+  }
+  void pushCostBlobs(...)
+  {
+  }
+  template <class C>
+  static auto bindCostEngine(C* c, mppib_engine* e) -> decltype(c->bindEngine(e), void())
+  {
+    if (c)
+      c->bindEngine(e);
+  }
+  static void bindCostEngine(...)
   {
   }
   // one engine solve for all distributions; x0s [D][S], Us [D][T][C] in the engine's layout

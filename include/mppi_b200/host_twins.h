@@ -9,7 +9,7 @@
  *   mppib_host_step_lstm / mppib_host_output_trajectory_lstm   the same two for RacerDubinsElevationLSTMSteering
  *   mppib_host_free_energy          mppi::kernels::computeFreeEnergy      include/mppi/core/mppi_common.cu:1065-1081
  *   mppib_host_merge_records        (no reference counterpart: the log-sum-exp merge of rollout shards, SURVEY §8e)
- *   mppib_host_state_cost           the robust costs' host computeStateCost / getStabilizingCost / getCostmapCost (below)
+ *   mppib_host_state_cost           the robust costs' and QuadrotorMapCost's host computeStateCost and terms (below)
  * Arrays: u / history are [T][C] / [2][C] (== Eigen C x T / C x 2 column-major), states [T][S], outputs [T][O].
  */
 #ifndef MPPI_B200_HOST_TWINS_H_
@@ -94,12 +94,35 @@ int mppib_host_npz_read(const char* path, const char* name, float* out, size_t c
  *                         0.1 * crash_cost); the rollouts use the device body's 0.5 / 0.5 * crash_cost, as in the reference
  *   MPPIB_COST_AR_ROBUST  ar_robust_cost.cu:13-132, host branch: cosf / sinf and the nearest texel (std::round after the
  *                         clamps of :64-70); costmap = float4 per texel, row-major [map_height][map_width]
- * `params` is the cost's parameter blob (params.h). Other cost ids: MPPIB_ERR_UNSUPPORTED. Neither cost reads t or crash. */
+ *   MPPIB_COST_QUADROTOR_MAP  quadrotor_map_cost.cu:63-90, the host body: gate side + height + heading + speed +
+ *                         stabilizing + waypoint terms and the gate-pass term; no costmap term and no crash flag (the
+ *                         rollouts use the device body, :92-144). `costmap` is not read.
+ * `params` is the cost's parameter blob (params.h). Other cost ids: MPPIB_ERR_UNSUPPORTED. No cost reads t or crash. */
 int mppib_host_state_cost(int cost_id, const void* params, const float* costmap, const float* y, int t, int* crash,
                           float* cost);
 int mppib_host_ar_robust_stabilizing_cost(const mppib_ar_robust_cost_params* params, const float* s, float* cost);
 int mppib_host_ar_robust_costmap_cost(const mppib_ar_robust_cost_params* params, const float* costmap, const float* s,
                                       float* cost);
+/* QuadrotorMapCost's __host__ __device__ terms (quadrotor_map_cost.cu:199-357), host side, one per `term`; an unknown
+ * term is MPPIB_ERR_INVALID_ARG. distToWaypoint (:146-152) takes the waypoint as (x, y, z[, heading]). */
+enum mppib_quadrotor_map_term
+{
+  MPPIB_QMAP_GATE_SIDE = 0,   /* computeGateSideCost    :264-323 */
+  MPPIB_QMAP_HEADING = 1,     /* computeHeadingCost     :210-238 */
+  MPPIB_QMAP_HEIGHT = 2,      /* computeHeightCost      :325-357 */
+  MPPIB_QMAP_SPEED = 3,       /* computeSpeedCost       :240-252 */
+  MPPIB_QMAP_STABILIZING = 4, /* computeStabilizingCost :199-208 */
+  MPPIB_QMAP_WAYPOINT = 5     /* computeWaypointCost    :254-262 */
+};
+int mppib_host_quadrotor_map_term(const mppib_quadrotor_map_cost_params* params, int term, const float* s, float* cost);
+float mppib_host_quadrotor_map_dist_to_waypoint(const float* s, const float* waypoint);
+/* QuadrotorMapCostParams::updateWaypoint / updateGateBoundaries (quadrotor_map_cost.cuh:62-90): shift curr -> prev and set
+ * the new values (updateWaypoint derives the gate corners x +- cosf(heading) gate_width, y +- sinf(heading) gate_width).
+ * Return 1 if anything changed, 0 if not (the cost pushes its parameters only then), MPPIB_ERR_INVALID_ARG for NULL. Both
+ * the C++ and the Python mirror call these, so they produce the same bytes. */
+int mppib_host_quadrotor_map_update_waypoint(mppib_quadrotor_map_cost_params* p, float x, float y, float z, float heading);
+int mppib_host_quadrotor_map_update_gate_boundaries(mppib_quadrotor_map_cost_params* p, float left_x, float left_y,
+                                                    float left_z, float right_x, float right_y, float right_z);
 #ifdef __cplusplus
 }
 #endif

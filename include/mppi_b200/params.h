@@ -37,6 +37,7 @@ enum mppib_cost_id
   MPPIB_COST_QUADROTOR_QUADRATIC = 4, /* cost_functions/quadrotor/quadrotor_quadratic_cost.cuh */
   MPPIB_COST_DI_ROBUST = 5,          /* cost_functions/double_integrator/double_integrator_robust_cost.cuh (circle params) */
   MPPIB_COST_AR_ROBUST = 6,          /* cost_functions/autorally/ar_robust_cost.cuh */
+  MPPIB_COST_QUADROTOR_MAP = 7,      /* cost_functions/quadrotor/quadrotor_map_cost.cuh (map: MPPIB_BLOB_COST_TEXTURE) */
   MPPIB_COST_COUNT
 };
 
@@ -287,6 +288,38 @@ typedef struct mppib_quadrotor_cost_params
   float w_coeff;                                   /* 1 */
   float terminal_cost_coeff;                       /* 0 */
 } mppib_quadrotor_cost_params;
+
+/* QuadrotorMapCostParams (cost_functions/quadrotor/quadrotor_map_cost.cuh:14-91) without r_c1 / r_c2 / trs, which only
+ * the reference's float4 track texture reads and no cost body does. float4 waypoints are (x, y, z, heading), float3
+ * gate corners (x, y, z). The cost's map is TwoDTextureHelper<float> map 0 and travels as MPPIB_BLOB_COST_TEXTURE in
+ * the mppib_elevation_map_header format; without it the costmap term is 0 (checkTextureUse(0) false). */
+typedef struct mppib_quadrotor_map_cost_params
+{
+  float control_cost_coeff[MPPIB_MAX_CONTROL_DIM]; /* 1, 1, 1, 1 */
+  float discount;                                  /* CostParams default 1.0 (unused by this cost) */
+  float attitude_coeff;                            /* 10 */
+  float crash_coeff;                               /* 1000 */
+  float dist_to_waypoint_coeff;                    /* 0 */
+  float heading_coeff;                             /* 5 */
+  float heading_power;                             /* 1 */
+  float height_coeff;                              /* 5 */
+  float track_coeff;                               /* 10 */
+  float speed_coeff;                               /* 5 */
+  float track_slop;                                /* 0 */
+  float gate_pass_cost;                            /* -150 */
+  float curr_waypoint[4];                          /* 0, 0, 0, 0 */
+  float prev_waypoint[4];                          /* 0, 0, 0, 0 */
+  float curr_gate_left[3];                         /* 0, 0, 0 */
+  float curr_gate_right[3];                        /* 0, 0, 0 */
+  float prev_gate_left[3];                         /* 0, 0, 0 */
+  float prev_gate_right[3];                        /* 0, 0, 0 */
+  float end_waypoint[4];                           /* NaN x 4 (unused by the cost bodies) */
+  float desired_speed;                             /* 5 m/s */
+  float gate_margin;                               /* 0.5 m */
+  float min_dist_to_gate_side;                     /* 0.5 m */
+  float track_boundary_cost;                       /* 2.5 */
+  float gate_width;                                /* 2.15 m */
+} mppib_quadrotor_map_cost_params;
 /* ---- Sampler parameter blob (sampling_distribution.cuh:14-29, gaussian.cuh:21-61) --------------- */
 typedef struct mppib_gaussian_params
 {

@@ -111,6 +111,7 @@ static const PairEntry kPairs[] = {
   make_entry<plugins::RacerLSTMDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_LSTM, MPPIB_COST_RACER_QUADRATIC),
   make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorQuadraticCost>(MPPIB_DYN_QUADROTOR,
                                                                           MPPIB_COST_QUADROTOR_QUADRATIC),
+  make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorMapCost>(MPPIB_DYN_QUADROTOR, MPPIB_COST_QUADROTOR_MAP),
 };
 
 // RacerDubinsElevationLSTMSteering with the steering LSTM on tensor cores (hidden_dim 32, head width <= 24)
@@ -1153,6 +1154,7 @@ int mppib_destroy(mppib_engine* e)
   cudaFree(e->nn_theta_d);
   cudaFree(e->lstm_theta_d);
   cudaFree(e->elev_d);
+  cudaFree(e->cost_tex_d);
   cudaFree(e->fb_gains_d);
   cudaFree(e->ddp_ws_d);
   cudaFree(e->ddp_status_d);
@@ -1218,6 +1220,43 @@ int mppib_destroy(mppib_engine* e)
   return MPPIB_OK;
 }
 
+// A TwoDTextureHelper<float> map in the mppib_elevation_map_header + row-major floats format (params.h): validates the
+// header, grows the device buffer when needed and copies the values. Used by both map blobs (the RACER models' elevation
+// map and QuadrotorMapCost's costmap); `what` names the blob in the error text.
+static int upload_map_blob(mppib_engine& e, const char* what, const void* host, size_t nbytes, float*& data_d,
+                           size_t& capacity, mppib_elevation_map_header& hdr)
+{
+  if (nbytes < sizeof(mppib_elevation_map_header))
+    return fail(MPPIB_ERR_INVALID_ARG, "%s: %zu bytes is smaller than its header", what, nbytes);
+  mppib_elevation_map_header h;
+  memcpy(&h, host, sizeof(h));
+  if (h.width < 2 || h.height < 2 || h.width > 16384 || h.height > 16384)
+    return fail(MPPIB_ERR_INVALID_ARG, "%s: extent %d x %d (need 2 .. 16384 cells per side)", what, h.width, h.height);
+  const size_t cells = (size_t)h.width * h.height;
+  if (nbytes != sizeof(h) + cells * sizeof(float))
+    return fail(MPPIB_ERR_INVALID_ARG, "%s: got %zu bytes, expected %zu (header + %d x %d floats)", what, nbytes,
+                sizeof(h) + cells * sizeof(float), h.width, h.height);
+  for (int i = 0; i < 3; i++)
+    if (!std::isfinite(h.origin[i]) || !std::isfinite(h.resolution[i]) || h.resolution[i] == 0.0f)
+      return fail(MPPIB_ERR_INVALID_ARG, "%s: origin / resolution component %d is not usable", what, i);
+  for (int i = 0; i < 9; i++)
+    if (!std::isfinite(h.rotations[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "%s: rotation entry %d is not finite", what, i);
+  if (cells > capacity)
+  {
+    CUDA_TRY(cudaStreamSynchronize(e.stream));
+    cudaFree(data_d);
+    data_d = nullptr;
+    capacity = 0;
+    CUDA_TRY(cudaMalloc(&data_d, cells * sizeof(float)));
+    capacity = cells;
+  }
+  CUDA_TRY(cudaMemcpyAsync(data_d, (const char*)host + sizeof(h), cells * sizeof(float), cudaMemcpyHostToDevice, e.stream));
+  CUDA_TRY(cudaStreamSynchronize(e.stream));
+  hdr = h;
+  return MPPIB_OK;
+}
+
 int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
 {
   if (!e || !host)
@@ -1226,7 +1265,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
   // weights, the costmap texture and the LSTM blob are read by kernels of a solve still in flight (mppib_solve_async):
   // replacing them under it would be a use-after-free
   if (e->pending != 0 && (which == MPPIB_BLOB_NN_WEIGHTS || which == MPPIB_BLOB_LSTM_WEIGHTS || which == MPPIB_BLOB_COSTMAP ||
-                          which == MPPIB_BLOB_ELEVATION_MAP))
+                          which == MPPIB_BLOB_ELEVATION_MAP || which == MPPIB_BLOB_COST_TEXTURE))
     return fail(MPPIB_ERR_STATE, "mppib_set_blob(%d) while a solve is pending: call mppib_solve_wait first", which);
   switch (which)
   {
@@ -1354,39 +1393,18 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
       // copyToDevice of the RACER models' map 0 (racer_dubins_elevation.cuh: tex_helper_), in one blob
       if (e->desc.dynamics_id != MPPIB_DYN_RACER_LSTM)
         return fail(MPPIB_ERR_INVALID_ARG, "elevation map given to a dynamics without one");
-      if (nbytes < sizeof(mppib_elevation_map_header))
-        return fail(MPPIB_ERR_INVALID_ARG, "elevation map: %zu bytes is smaller than its header", nbytes);
-      mppib_elevation_map_header h;
-      memcpy(&h, host, sizeof(h));
-      if (h.width < 2 || h.height < 2 || h.width > 16384 || h.height > 16384)
-        return fail(MPPIB_ERR_INVALID_ARG, "elevation map: extent %d x %d (need 2 .. 16384 cells per side)", h.width, h.height);
-      const size_t cells = (size_t)h.width * h.height;
-      if (nbytes != sizeof(h) + cells * sizeof(float))
-        return fail(MPPIB_ERR_INVALID_ARG, "elevation map: got %zu bytes, expected %zu (header + %d x %d floats)", nbytes,
-                    sizeof(h) + cells * sizeof(float), h.width, h.height);
-      for (int i = 0; i < 3; i++)
-        if (!std::isfinite(h.origin[i]) || !std::isfinite(h.resolution[i]) || h.resolution[i] == 0.0f)
-          return fail(MPPIB_ERR_INVALID_ARG, "elevation map: origin / resolution component %d is not usable", i);
-      for (int i = 0; i < 9; i++)
-        if (!std::isfinite(h.rotations[i]))
-          return fail(MPPIB_ERR_INVALID_ARG, "elevation map: rotation entry %d is not finite", i);
       // the values themselves may be NaN (unobserved cells): the model's own isfinite guards handle that (racer_dubins.cu:414-425)
-      if (cells > e->elev_capacity)
-      {
-        CUDA_TRY(cudaStreamSynchronize(e->stream));
-        cudaFree(e->elev_d);
-        e->elev_d = nullptr;
-        e->elev_capacity = 0;
-        CUDA_TRY(cudaMalloc(&e->elev_d, cells * sizeof(float)));
-        e->elev_capacity = cells;
-      }
-      CUDA_TRY(cudaMemcpyAsync(e->elev_d, (const char*)host + sizeof(h), cells * sizeof(float), cudaMemcpyHostToDevice,
-                               e->stream));
-      CUDA_TRY(cudaStreamSynchronize(e->stream));
-      e->elev_hdr = h;
+      const int rc = upload_map_blob(*e, "elevation map", host, nbytes, e->elev_d, e->elev_capacity, e->elev_hdr);
+      if (rc != MPPIB_OK)
+        return rc;
       e->elev_h.assign((const unsigned char*)host, (const unsigned char*)host + nbytes);
       return MPPIB_OK;
     }
+    case MPPIB_BLOB_COST_TEXTURE:
+      // QuadrotorMapCost's tex_helper_ map 0 (quadrotor_map_cost.cu:37-61), the same format
+      if (e->desc.cost_id != MPPIB_COST_QUADROTOR_MAP)
+        return fail(MPPIB_ERR_INVALID_ARG, "cost texture given to a cost without one");
+      return upload_map_blob(*e, "cost texture", host, nbytes, e->cost_tex_d, e->cost_tex_capacity, e->cost_tex_hdr);
     case MPPIB_BLOB_COSTMAP:
     {
       if (!cost_has_map(e->desc.cost_id))

@@ -143,6 +143,9 @@ struct mppib_engine
   std::vector<unsigned char> elev_h;
   size_t elev_capacity = 0;              // floats allocated
   mppib_elevation_map_header elev_hdr{};  // use == 0 until a map is set
+  float* cost_tex_d = nullptr;               // MPPIB_BLOB_COST_TEXTURE: QuadrotorMapCost's map, width * height floats
+  size_t cost_tex_capacity = 0;              // floats allocated
+  mppib_elevation_map_header cost_tex_hdr{};  // use == 0 until a map is set
   cudaArray_t costmap_array = nullptr;
   cudaTextureObject_t costmap_tex = 0;
 
@@ -284,6 +287,18 @@ struct AuxFill<plugins::ARStandardCost::Aux>
   static void fill(plugins::ARStandardCost::Aux& a, const mppib_engine& e)
   {
     a.costmap_tex = e.costmap_tex;
+  }
+};
+
+template <>
+struct AuxFill<plugins::QuadrotorMapCost::Aux>
+{
+  static void fill(plugins::QuadrotorMapCost::Aux& a, const mppib_engine& e)
+  {
+    a.map.data = e.cost_tex_d;
+    a.map.hdr = e.cost_tex_hdr;
+    if (!e.cost_tex_d)
+      a.map.hdr.use = 0;
   }
 };
 

@@ -663,6 +663,97 @@ float ar_robust_costmap_cost(const mppib_ar_robust_cost_params& p, const float* 
   return cost;
 }
 
+// ---- QuadrotorMapCost (quadrotor_map_cost.cu), the __host__ side of its __host__ __device__ terms -------------------
+using QMapParams = mppib_quadrotor_map_cost_params;
+// :146-152
+float qmap_dist_to_waypoint(const float* s, const float* w)
+{
+  return std::sqrt((s[0] - w[0]) * (s[0] - w[0]) + (s[1] - w[1]) * (s[1] - w[1]) + (s[2] - w[2]) * (s[2] - w[2]));
+}
+// :264-323
+float qmap_gate_side_cost(const QMapParams& p, const float* s)
+{
+  float cost = 0;
+  const float gx = p.curr_gate_left[0] - p.curr_gate_right[0], gy = p.curr_gate_left[1] - p.curr_gate_right[1];
+  const float rx = s[0] - p.curr_gate_right[0], ry = s[1] - p.curr_gate_right[1];
+  const float perp_dist = rx * gy - ry * gx;
+  const float comp = (rx * gx + ry * gy) / (gx * gx + gy * gy);
+  if (std::fabs(perp_dist) < p.min_dist_to_gate_side && ((comp < 0.0f && comp >= -0.5f) || (comp > 1.0f && comp <= 1.5f)))
+    cost += p.crash_coeff * std::fabs(comp);
+  return cost;
+}
+// :325-357: double weights and interpolation narrowed to float; +400 when the squared difference exceeds gate_width
+float qmap_height_cost(const QMapParams& p, const float* s)
+{
+  float cost = 0;
+  float d1 = sqrtf((s[0] - p.prev_waypoint[0]) * (s[0] - p.prev_waypoint[0]) +
+                   (s[1] - p.prev_waypoint[1]) * (s[1] - p.prev_waypoint[1]));
+  float d2 = sqrtf((s[0] - p.curr_waypoint[0]) * (s[0] - p.curr_waypoint[0]) +
+                   (s[1] - p.curr_waypoint[1]) * (s[1] - p.curr_waypoint[1]));
+  float w1 = d1 / (d1 + d2 + 0.001);
+  float w2 = d2 / (d1 + d2 + 0.001);
+  float interpolated_height = (1.0 - w1) * p.prev_waypoint[2] + (1.0 - w2) * p.curr_waypoint[2];
+  float dz = std::fabs(s[2] - interpolated_height);
+  float height_diff = dz * dz;
+  cost += p.height_coeff * height_diff;
+  if (height_diff > p.gate_width)
+    cost += 400;
+  return cost;
+}
+// :210-238
+float qmap_heading_cost(const QMapParams& p, const float* s)
+{
+  float cost = 0;
+  const float* q = s + 6;
+  const float vx = s[3], vy = s[4], vz = s[5];
+  const float R00 = q[0] * q[0] + q[1] * q[1] - q[2] * q[2] - q[3] * q[3];
+  const float R01 = 2 * (q[1] * q[2] - q[0] * q[3]);
+  const float R02 = 2 * (q[1] * q[3] + q[0] * q[2]);
+  const float R10 = 2 * (q[1] * q[2] + q[0] * q[3]);
+  const float R11 = q[0] * q[0] - q[1] * q[1] + q[2] * q[2] - q[3] * q[3];
+  const float R12 = 2 * (q[2] * q[3] - q[0] * q[1]);
+  const float yaw = atan2f(R10 * vx + R11 * vy + R12 * vz, R00 * vx + R01 * vy + R02 * vz);
+  const float w_heading = atan2f(p.curr_waypoint[1] - s[1], p.curr_waypoint[0] - s[0]);
+  if (qmap_dist_to_waypoint(s, p.curr_waypoint) > p.gate_margin)
+    cost += p.heading_coeff * powf(std::fabs(normalize_angle(yaw - w_heading)), p.heading_power);
+  return cost;
+}
+// :240-252
+float qmap_speed_cost(const QMapParams& p, const float* s)
+{
+  const float speed = std::sqrt(s[3] * s[3] + s[4] * s[4]);
+  return p.speed_coeff * ((speed - p.desired_speed) * (speed - p.desired_speed));
+}
+// :199-208 with Quat2EulerNWU (math_utils.h:263-270)
+float qmap_stabilizing_cost(const QMapParams& p, const float* s)
+{
+  const float* q = s + 6;
+  const float roll = atan2f(2.0f * q[3] * q[2] + 2.0f * q[0] * q[1], q[0] * q[0] + q[3] * q[3] - q[2] * q[2] - q[1] * q[1]);
+  const float temp = -2.0f * q[0] * q[2] + 2.0f * q[1] * q[3];
+  const float pitch = -asinf(fmaxf(fminf(1.0f, temp), -1.0f));
+  return p.attitude_coeff * (roll * roll + pitch * pitch);
+}
+// :254-262
+float qmap_waypoint_cost(const QMapParams& p, const float* s)
+{
+  const float d = qmap_dist_to_waypoint(s, p.curr_waypoint);
+  return p.dist_to_waypoint_coeff * (d * d);
+}
+// :63-90, the HOST body: no costmap term, no crash flag, and the waypoint term added (the device body is in costs.cuh)
+float qmap_state_cost(const QMapParams& p, const float* s)
+{
+  float cost = 0;
+  cost += qmap_gate_side_cost(p, s);
+  cost += qmap_height_cost(p, s);
+  cost += qmap_heading_cost(p, s);
+  cost += qmap_speed_cost(p, s);
+  cost += qmap_stabilizing_cost(p, s);
+  cost += qmap_waypoint_cost(p, s);
+  if (qmap_dist_to_waypoint(s, p.curr_waypoint) < p.gate_margin)
+    cost += p.gate_pass_cost;
+  return cost;
+}
+
 }  // namespace
 
 extern "C" {
@@ -671,7 +762,7 @@ int mppib_host_state_cost(int cost_id, const void* params, const float* costmap,
                           float* cost)
 {
   (void)t;
-  (void)crash;  // neither robust cost reads the time step or the crash flag
+  (void)crash;  // no host body reads the time step or the crash flag
   if (!params || !y || !cost)
     return MPPIB_ERR_INVALID_ARG;
   switch (cost_id)
@@ -690,9 +781,80 @@ int mppib_host_state_cost(int cost_id, const void* params, const float* costmap,
       *cost = c;
       return MPPIB_OK;
     }
+    case MPPIB_COST_QUADROTOR_MAP:
+      *cost = qmap_state_cost(*static_cast<const mppib_quadrotor_map_cost_params*>(params), y);
+      return MPPIB_OK;
     default:
       return MPPIB_ERR_UNSUPPORTED;
   }
+}
+
+int mppib_host_quadrotor_map_term(const mppib_quadrotor_map_cost_params* params, int term, const float* s, float* cost)
+{
+  if (!params || !s || !cost)
+    return MPPIB_ERR_INVALID_ARG;
+  const mppib_quadrotor_map_cost_params& p = *params;
+  switch (term)
+  {
+    case MPPIB_QMAP_GATE_SIDE:
+      *cost = qmap_gate_side_cost(p, s);
+      return MPPIB_OK;
+    case MPPIB_QMAP_HEADING:
+      *cost = qmap_heading_cost(p, s);
+      return MPPIB_OK;
+    case MPPIB_QMAP_HEIGHT:
+      *cost = qmap_height_cost(p, s);
+      return MPPIB_OK;
+    case MPPIB_QMAP_SPEED:
+      *cost = qmap_speed_cost(p, s);
+      return MPPIB_OK;
+    case MPPIB_QMAP_STABILIZING:
+      *cost = qmap_stabilizing_cost(p, s);
+      return MPPIB_OK;
+    case MPPIB_QMAP_WAYPOINT:
+      *cost = qmap_waypoint_cost(p, s);
+      return MPPIB_OK;
+    default:
+      return MPPIB_ERR_INVALID_ARG;
+  }
+}
+
+int mppib_host_quadrotor_map_update_gate_boundaries(mppib_quadrotor_map_cost_params* p, float left_x, float left_y,
+                                                    float left_z, float right_x, float right_y, float right_z)
+{
+  if (!p)
+    return MPPIB_ERR_INVALID_ARG;
+  if (p->curr_gate_left[0] != left_x || p->curr_gate_left[1] != left_y || p->curr_gate_left[2] != left_z ||
+      p->curr_gate_right[0] != right_x || p->curr_gate_right[1] != right_y || p->curr_gate_right[2] != right_z)
+  {
+    memcpy(p->prev_gate_left, p->curr_gate_left, sizeof(p->prev_gate_left));
+    memcpy(p->prev_gate_right, p->curr_gate_right, sizeof(p->prev_gate_right));
+    p->curr_gate_left[0] = left_x, p->curr_gate_left[1] = left_y, p->curr_gate_left[2] = left_z;
+    p->curr_gate_right[0] = right_x, p->curr_gate_right[1] = right_y, p->curr_gate_right[2] = right_z;
+    return 1;
+  }
+  return 0;
+}
+
+int mppib_host_quadrotor_map_update_waypoint(mppib_quadrotor_map_cost_params* p, float x, float y, float z, float heading)
+{
+  if (!p)
+    return MPPIB_ERR_INVALID_ARG;
+  if (p->curr_waypoint[0] != x || p->curr_waypoint[1] != y || p->curr_waypoint[2] != z || p->curr_waypoint[3] != heading)
+  {
+    memcpy(p->prev_waypoint, p->curr_waypoint, sizeof(p->prev_waypoint));
+    p->curr_waypoint[0] = x, p->curr_waypoint[1] = y, p->curr_waypoint[2] = z, p->curr_waypoint[3] = heading;
+    const float w = p->gate_width;
+    mppib_host_quadrotor_map_update_gate_boundaries(p, x + cosf(heading) * w, y + sinf(heading) * w, z,
+                                                    x - cosf(heading) * w, y - sinf(heading) * w, z);
+    return 1;
+  }
+  return 0;
+}
+
+float mppib_host_quadrotor_map_dist_to_waypoint(const float* s, const float* waypoint)
+{
+  return (s && waypoint) ? qmap_dist_to_waypoint(s, waypoint) : 0.0f;
 }
 
 int mppib_host_ar_robust_stabilizing_cost(const mppib_ar_robust_cost_params* params, const float* s, float* cost)

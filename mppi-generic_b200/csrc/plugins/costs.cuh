@@ -7,6 +7,7 @@
 #pragma once
 #include "../device_utils.cuh"
 #include "../../../include/mppi_b200/params.h"
+#include "texture_map.cuh"
 
 namespace mppib
 {
@@ -438,6 +439,133 @@ struct QuadrotorQuadraticCost : public Cost<QuadrotorQuadraticCost, mppib_quadro
   __device__ static __forceinline__ float terminalCost(const Params& p, const Aux& a, const float* s)
   {
     return p.terminal_cost_coeff * computeStateCost(p, a, nullptr, s, 0, nullptr);
+  }
+};
+
+// cost_functions/quadrotor/quadrotor_map_cost.cu:92-144 (device body; terminalCost :397-407 == 0) with the float-array
+// helpers Quat2EulerNWU / Quat2DCM of utils/math_utils.h:263-283 and angle_utils::shortestAngularDistance. The reference's
+// host body (:63-90) is another function: no costmap term, no crash flag, and computeWaypointCost added. It is restated in
+// host_twins.cpp, each side keeping its own (DESIGN.md §8). The device printf calls of the gate and map terms are not
+// restated. The map is tex_helper_'s map 0 (MPPIB_BLOB_COST_TEXTURE), read through texture_map.cuh.
+struct QuadrotorMapCost : public Cost<QuadrotorMapCost, mppib_quadrotor_map_cost_params>
+{
+  struct Aux
+  {
+    ElevationMap map;  // hdr.use == 0: no map, the costmap term is 0 (checkTextureUse(0) false)
+  };
+  __device__ static __forceinline__ void initializeCosts(const Params&, const Aux&, float*, int)
+  {
+  }
+  // :146-152: sqrt of a float sum
+  __device__ static __forceinline__ float distToWaypoint(const float* s, const float* w)
+  {
+    return sqrtf(MPPIB_SQ(s[0] - w[0]) + MPPIB_SQ(s[1] - w[1]) + MPPIB_SQ(s[2] - w[2]));
+  }
+  // :359-395. Outside [0, 1] of the normalised map adds crash_coeff directly (not through the flag), and the clamped map
+  // is still read.
+  __device__ static __forceinline__ float computeCostmapCost(const Params& p, const Aux& aux, const float* s)
+  {
+    float cost = 0;
+    if (!aux.map.hdr.use)
+      return cost;
+    const float2 tc = worldPoseToTexCoord(aux.map.hdr, s[0], s[1], s[2]);
+    if (tc.x < 0.0f || tc.x > 1.0f || tc.y < 0.0f || tc.y > 1.0f)
+      cost += p.crash_coeff;
+    const float track_cost =
+        queryTextureBilinear(aux.map, tc.x * (float)aux.map.hdr.width - 0.5f, tc.y * (float)aux.map.hdr.height - 0.5f);
+    if (track_cost > p.track_slop)
+      cost += p.track_coeff * track_cost;
+    if (track_cost > p.track_boundary_cost)
+      cost += p.crash_coeff;
+    return cost;
+  }
+  // :264-323. Only the along-gate component from the right corner and the cross product are used; it fires within
+  // min_dist_to_gate_side of the gate line, in the bands [-0.5, 0) and (1, 1.5] along it.
+  __device__ static __forceinline__ float computeGateSideCost(const Params& p, const float* s)
+  {
+    float cost = 0;
+    const float gx = p.curr_gate_left[0] - p.curr_gate_right[0], gy = p.curr_gate_left[1] - p.curr_gate_right[1];
+    const float rx = s[0] - p.curr_gate_right[0], ry = s[1] - p.curr_gate_right[1];
+    const float perp_dist = rx * gy - ry * gx;
+    const float comp = (rx * gx + ry * gy) / (gx * gx + gy * gy);
+    if (fabsf(perp_dist) < p.min_dist_to_gate_side &&
+        ((comp < 0.0f && comp >= -0.5f) || (comp > 1.0f && comp <= 1.5f)))
+      cost += p.crash_coeff * fabsf(comp);
+    return cost;
+  }
+  // :325-357. The weights and the interpolated height are double operations (the literals 0.001 and 1.0) narrowed to
+  // float; the `height_diff < 0` branch of the reference is dead (a square), and +400 is added when the SQUARED height
+  // difference exceeds gate_width.
+  __device__ static __forceinline__ float computeHeightCost(const Params& p, const float* s)
+  {
+    float cost = 0;
+    const float d1 = sqrtf(MPPIB_SQ(s[0] - p.prev_waypoint[0]) + MPPIB_SQ(s[1] - p.prev_waypoint[1]));
+    const float d2 = sqrtf(MPPIB_SQ(s[0] - p.curr_waypoint[0]) + MPPIB_SQ(s[1] - p.curr_waypoint[1]));
+    const float w1 = (float)((double)d1 / ((double)(d1 + d2) + 0.001));
+    const float w2 = (float)((double)d2 / ((double)(d1 + d2) + 0.001));
+    const float interpolated_height =
+        (float)((1.0 - (double)w1) * (double)p.prev_waypoint[2] + (1.0 - (double)w2) * (double)p.curr_waypoint[2]);
+    const float height_diff = MPPIB_SQ(fabsf(s[2] - interpolated_height));
+    cost += p.height_coeff * height_diff;
+    if (height_diff > p.gate_width)
+      cost += 400;
+    return cost;
+  }
+  // :210-238: the yaw of the world-frame velocity Quat2DCM(q) v against the bearing to the waypoint, outside gate_margin
+  __device__ static __forceinline__ float computeHeadingCost(const Params& p, const float* s)
+  {
+    float cost = 0;
+    const float* q = s + 6;
+    const float vx = s[3], vy = s[4], vz = s[5];
+    const float R00 = MPPIB_SQ(q[0]) + MPPIB_SQ(q[1]) - MPPIB_SQ(q[2]) - MPPIB_SQ(q[3]);
+    const float R01 = 2 * (q[1] * q[2] - q[0] * q[3]);
+    const float R02 = 2 * (q[1] * q[3] + q[0] * q[2]);
+    const float R10 = 2 * (q[1] * q[2] + q[0] * q[3]);
+    const float R11 = MPPIB_SQ(q[0]) - MPPIB_SQ(q[1]) + MPPIB_SQ(q[2]) - MPPIB_SQ(q[3]);
+    const float R12 = 2 * (q[2] * q[3] - q[0] * q[1]);
+    const float yaw = atan2f(R10 * vx + R11 * vy + R12 * vz, R00 * vx + R01 * vy + R02 * vz);
+    const float w_heading = atan2f(p.curr_waypoint[1] - s[1], p.curr_waypoint[0] - s[0]);
+    if (distToWaypoint(s, p.curr_waypoint) > p.gate_margin)
+      cost += p.heading_coeff * powf(fabsf(normalizeAngle(yaw - w_heading)), p.heading_power);
+    return cost;
+  }
+  // :240-252
+  __device__ static __forceinline__ float computeSpeedCost(const Params& p, const float* s)
+  {
+    const float speed = sqrtf(s[3] * s[3] + s[4] * s[4]);
+    return p.speed_coeff * MPPIB_SQ(speed - p.desired_speed);
+  }
+  // :199-208: roll and pitch of Quat2EulerNWU
+  __device__ static __forceinline__ float computeStabilizingCost(const Params& p, const float* s)
+  {
+    const float* q = s + 6;
+    const float roll = atan2f(2.0f * q[3] * q[2] + 2.0f * q[0] * q[1], q[0] * q[0] + q[3] * q[3] - q[2] * q[2] - q[1] * q[1]);
+    const float temp = -2.0f * q[0] * q[2] + 2.0f * q[1] * q[3];
+    const float pitch = -asinf(fmaxf(fminf(1.0f, temp), -1.0f));
+    return p.attitude_coeff * (MPPIB_SQ(roll) + MPPIB_SQ(pitch));
+  }
+  // :92-144. computeWaypointCost is evaluated but not added on the device, so it is not computed here. A non-zero gate
+  // cost raises the sticky crash flag, which then adds crash_coeff at every later step of the sample.
+  __device__ static __forceinline__ float computeStateCost(const Params& p, const Aux& aux, const float*, const float* s,
+                                                           int, int* crash_status)
+  {
+    const float costmap_cost = computeCostmapCost(p, aux, s);
+    const float gate_cost = computeGateSideCost(p, s);
+    const float height_cost = computeHeightCost(p, s);
+    const float heading_cost = computeHeadingCost(p, s);
+    const float speed_cost = computeSpeedCost(p, s);
+    const float stable_cost = computeStabilizingCost(p, s);
+    if (gate_cost != 0)
+      *crash_status = 1;
+    float cost = costmap_cost + gate_cost + height_cost + heading_cost + speed_cost + stable_cost;
+    if (distToWaypoint(s, p.curr_waypoint) < p.gate_margin)
+      cost += p.gate_pass_cost;
+    cost += *crash_status * p.crash_coeff;
+    return cost;
+  }
+  __device__ static __forceinline__ float terminalCost(const Params&, const Aux&, const float*)
+  {
+    return 0.0f;
   }
 };
 

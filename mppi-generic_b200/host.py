@@ -12,6 +12,8 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
+import sys
+import weakref
 from typing import Optional, Sequence
 
 import numpy as np
@@ -28,8 +30,12 @@ FLT_MAX = 3.4028234663852886e38
 DYN_CARTPOLE, DYN_DOUBLE_INTEGRATOR, DYN_AUTORALLY_NN, DYN_RACER_LSTM, DYN_QUADROTOR = 0, 1, 2, 3, 4
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
 COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
+COST_QUADROTOR_MAP = 7
 SAMPLER_GAUSSIAN, SAMPLER_COLORED_NOISE, SAMPLER_NLN = 0, 1, 2
 BLOB_DYN, BLOB_COST, BLOB_SAMPLER, BLOB_NN_WEIGHTS, BLOB_COSTMAP, BLOB_LSTM_WEIGHTS, BLOB_ELEVATION_MAP = range(7)
+BLOB_COST_TEXTURE = 7
+# QuadrotorMapCost's terms (host_twins.h: mppib_quadrotor_map_term)
+QMAP_GATE_SIDE, QMAP_HEADING, QMAP_HEIGHT, QMAP_SPEED, QMAP_STABILIZING, QMAP_WAYPOINT = range(6)
 FLAG_WRITEBACK_CONTROLS, FLAG_NO_TMA, FLAG_CURAND_HOST_API, FLAG_NO_PREFETCH, FLAG_NN_TENSOR, FLAG_RMPPI = 1, 2, 4, 8, 16, 32
 FLAG_NN_MMA, FLAG_NN_FFMA2 = 64, 128
 FLAG_NO_WARP_SPEC = 256
@@ -98,6 +104,46 @@ class QuadrotorCostParams(C.Structure):
                 ("x_coeff", C.c_float), ("v_coeff", C.c_float), ("use_euler", C.c_int), ("q_coeff", C.c_float),
                 ("roll_coeff", C.c_float), ("pitch_coeff", C.c_float), ("yaw_coeff", C.c_float),
                 ("w_coeff", C.c_float), ("terminal_cost_coeff", C.c_float)]
+
+
+class QuadrotorMapCostParams(C.Structure):
+    """mppib_quadrotor_map_cost_params (params.h): QuadrotorMapCostParams without r_c1 / r_c2 / trs. updateWaypoint /
+    updateGateBoundaries run in the library (mppib_host_quadrotor_map_update_*), so the C++ and Python mirrors write the same
+    bytes."""
+    _fields_ = [("control_cost_coeff", C.c_float * MAX_C), ("discount", C.c_float), ("attitude_coeff", C.c_float),
+                ("crash_coeff", C.c_float), ("dist_to_waypoint_coeff", C.c_float), ("heading_coeff", C.c_float),
+                ("heading_power", C.c_float), ("height_coeff", C.c_float), ("track_coeff", C.c_float),
+                ("speed_coeff", C.c_float), ("track_slop", C.c_float), ("gate_pass_cost", C.c_float),
+                ("curr_waypoint", C.c_float * 4), ("prev_waypoint", C.c_float * 4), ("curr_gate_left", C.c_float * 3),
+                ("curr_gate_right", C.c_float * 3), ("prev_gate_left", C.c_float * 3), ("prev_gate_right", C.c_float * 3),
+                ("end_waypoint", C.c_float * 4), ("desired_speed", C.c_float), ("gate_margin", C.c_float),
+                ("min_dist_to_gate_side", C.c_float), ("track_boundary_cost", C.c_float), ("gate_width", C.c_float)]
+
+    def set_defaults(self) -> None:
+        """quadrotor_map_cost.cuh:14-60."""
+        for i in range(MAX_C):
+            self.control_cost_coeff[i] = 1.0
+        self.discount = 1.0
+        self.attitude_coeff, self.crash_coeff, self.dist_to_waypoint_coeff = 10.0, 1000.0, 0.0
+        self.heading_coeff, self.heading_power, self.height_coeff = 5.0, 1.0, 5.0
+        self.track_coeff, self.speed_coeff, self.track_slop, self.gate_pass_cost = 10.0, 5.0, 0.0, -150.0
+        for i in range(4):
+            self.end_waypoint[i] = float("nan")
+        self.desired_speed, self.gate_margin, self.min_dist_to_gate_side = 5.0, 0.5, 0.5
+        self.track_boundary_cost, self.gate_width = 2.5, 2.15
+
+    def updateWaypoint(self, x: float, y: float, z: float, heading: float = 0.0) -> bool:
+        rc = lib().mppib_host_quadrotor_map_update_waypoint(C.byref(self), C.c_float(x), C.c_float(y), C.c_float(z),
+                                                            C.c_float(heading))
+        _check(min(rc, 0))
+        return rc == 1
+
+    def updateGateBoundaries(self, left_x: float, left_y: float, left_z: float, right_x: float, right_y: float,
+                             right_z: float) -> bool:
+        rc = lib().mppib_host_quadrotor_map_update_gate_boundaries(
+            C.byref(self), *[C.c_float(v) for v in (left_x, left_y, left_z, right_x, right_y, right_z)])
+        _check(min(rc, 0))
+        return rc == 1
 
 
 class RacerLSTMDynParams(C.Structure):
@@ -275,6 +321,8 @@ ABI_SYMBOLS = [
     "mppib_set_rmppi", "mppib_init_eval", "mppib_set_tsallis", "mppib_sample_trajectories", "mppib_nominal_trajectory", "mppib_compute_control", "mppib_host_npz_read", "mppib_comm_p2p_handle", "mppib_comm_p2p_open", "mppib_host_rmppi_line_search_weights", "mppib_host_rmppi_candidates",
     "mppib_host_rmppi_best_index", "mppib_set_ddp", "mppib_ddp_feedback",
     "mppib_host_state_cost", "mppib_host_ar_robust_stabilizing_cost", "mppib_host_ar_robust_costmap_cost",
+    "mppib_host_quadrotor_map_term", "mppib_host_quadrotor_map_dist_to_waypoint",
+    "mppib_host_quadrotor_map_update_waypoint", "mppib_host_quadrotor_map_update_gate_boundaries",
 ]
 
 _lib = None
@@ -324,6 +372,11 @@ def lib() -> C.CDLL:
     L.mppib_host_state_cost.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp]
     L.mppib_host_ar_robust_stabilizing_cost.argtypes = [vp, vp, vp]
     L.mppib_host_ar_robust_costmap_cost.argtypes = [vp, vp, vp, vp]
+    L.mppib_host_quadrotor_map_term.argtypes = [vp, C.c_int, vp, vp]
+    L.mppib_host_quadrotor_map_dist_to_waypoint.argtypes = [vp, vp]
+    L.mppib_host_quadrotor_map_dist_to_waypoint.restype = C.c_float
+    L.mppib_host_quadrotor_map_update_waypoint.argtypes = [vp] + [C.c_float] * 4
+    L.mppib_host_quadrotor_map_update_gate_boundaries.argtypes = [vp] + [C.c_float] * 6
     L.mppib_host_step.argtypes = [C.c_int, vp, vp, vp, vp, C.c_float, vp, vp, vp]
     L.mppib_host_smooth_controls.argtypes = [vp, vp, C.c_int, C.c_int]
     L.mppib_host_smooth_controls.restype = None
@@ -1050,6 +1103,94 @@ class QuadrotorQuadraticCost(_Cost):
         return np.array(list(self.params.s_goal), dtype=np.float32)
 
 
+class QuadrotorMapCost(_Cost):
+    """cost_functions/quadrotor/quadrotor_map_cost.cuh (defaults of :14-60 reproduced). The map is ``tex_helper_``'s map 0
+    (a TwoDTextureHelper), pushed with the cost's parameters as MPPIB_BLOB_COST_TEXTURE. computeStateCost and the
+    compute*Cost terms are the reference's HOST bodies; the rollouts run its device body, which adds the costmap term and
+    the crash flag and leaves the waypoint term out (DESIGN.md §8). updateWaypoint / updateGateBoundaries push to the
+    engines built on this cost only when something changed, as in the reference (quadrotor_map_cost.cu:161-196)."""
+    COST_ID = COST_QUADROTOR_MAP
+
+    def __init__(self):
+        super().__init__()
+        p = QuadrotorMapCostParams()
+        p.set_defaults()
+        self.params = p
+        self.tex_helper_ = TwoDTextureHelper()
+        self._engines = weakref.WeakSet()
+        self.params_pushes = 0  # paramsToDevice calls that reached an engine
+
+    def _bind_engine(self, engine) -> None:
+        self._engines.add(engine)
+
+    def paramsToDevice(self) -> None:
+        """The parameter blob and tex_helper_'s map to every open engine built on this cost."""
+        pushed = False
+        for e in list(self._engines):
+            if e._h:
+                e.push_cost()
+                pushed = True
+        if pushed:
+            self.params_pushes += 1
+
+    def updateWaypoint(self, x, y=None, z=None, heading: float = 0.0) -> None:
+        """updateWaypoint(float4) or updateWaypoint(x, y, z, heading = 0)."""
+        if y is None:
+            x, y, z, heading = (float(v) for v in x)
+        if self.params.updateWaypoint(x, y, z, heading):
+            self.paramsToDevice()
+
+    def updateGateBoundaries(self, *args) -> None:
+        """(left float3, right float3), (list of >= 6 floats) or (left_x, left_y, left_z, right_x, right_y, right_z)."""
+        if len(args) == 2:
+            vals = list(args[0])[:3] + list(args[1])[:3]
+        elif len(args) == 1:
+            vals = list(args[0])
+            if len(vals) < 6:  # quadrotor_map_cost.cu:176-181
+                print(f"You need {6 - len(vals)} more floats in the call to updateGateBoundaries", file=sys.stderr)
+                return
+        else:
+            vals = list(args)
+        if self.params.updateGateBoundaries(*[float(v) for v in vals[:6]]):
+            self.paramsToDevice()
+
+    def computeStateCost(self, y, t: int = 0, crash_status=None) -> float:
+        """quadrotor_map_cost.cu:63-90 (host body)."""
+        return _host_state_cost(self, y, t)
+
+    def terminalCost(self, y) -> float:
+        return 0.0
+
+    def _term(self, term: int, s) -> float:
+        out = C.c_float()
+        _check(lib().mppib_host_quadrotor_map_term(C.byref(self.params), term, _ptr(_f32(s)), C.byref(out)))
+        return out.value
+
+    def computeGateSideCost(self, s) -> float:
+        return self._term(QMAP_GATE_SIDE, s)
+
+    def computeHeadingCost(self, s) -> float:
+        return self._term(QMAP_HEADING, s)
+
+    def computeHeightCost(self, s) -> float:
+        return self._term(QMAP_HEIGHT, s)
+
+    def computeSpeedCost(self, s) -> float:
+        return self._term(QMAP_SPEED, s)
+
+    def computeStabilizingCost(self, s) -> float:
+        return self._term(QMAP_STABILIZING, s)
+
+    def computeWaypointCost(self, s) -> float:
+        return self._term(QMAP_WAYPOINT, s)
+
+    def distToWaypoint(self, s, waypoint) -> float:
+        L = lib()
+        L.mppib_host_quadrotor_map_dist_to_waypoint.restype = C.c_float
+        w = _f32(list(waypoint)[:3] + [0.0])
+        return float(L.mppib_host_quadrotor_map_dist_to_waypoint(_ptr(_f32(s)), _ptr(w)))
+
+
 class RacerQuadraticCost(_Cost):
     """Quadratic tracking cost on the RACER output vector (ours; params.h: mppib_racer_quadratic_cost_params)."""
     COST_ID = COST_RACER_QUADRATIC
@@ -1146,16 +1287,27 @@ class Engine:
             d.model_dims[i] = v
         _check(lib().mppib_create(C.byref(self._h), C.byref(d)))
         self.push_params()
+        if hasattr(cost, "_bind_engine"):
+            cost._bind_engine(self)
         nl, no = C.c_int(), C.c_int()
         _check(lib().mppib_local_rollouts(self._h, C.byref(nl), C.byref(no)))
         self.n_local, self.n_offset = nl.value, no.value
+
+    def push_cost(self) -> None:
+        """The cost's parameter blob, and QuadrotorMapCost's map (tex_helper_ map 0) when it has one."""
+        L = lib()
+        b = self.cost.blob()
+        _check(L.mppib_set_blob(self._h, BLOB_COST, b, len(b)))
+        if self.cost.COST_ID == COST_QUADROTOR_MAP:
+            m = self.cost.tex_helper_.blob()
+            if m is not None:
+                _check(L.mppib_set_blob(self._h, BLOB_COST_TEXTURE, m.ctypes.data, m.nbytes))
 
     def push_params(self) -> None:
         L = lib()
         b = self.dyn.blob()
         _check(L.mppib_set_blob(self._h, BLOB_DYN, b, len(b)))
-        b = self.cost.blob()
-        _check(L.mppib_set_blob(self._h, BLOB_COST, b, len(b)))
+        self.push_cost()
         b = self.sampler.blob()
         _check(L.mppib_set_blob(self._h, BLOB_SAMPLER, b, len(b)))
         if self.dyn.DYN_ID == DYN_AUTORALLY_NN:

@@ -232,6 +232,77 @@ def quadrotor(N: int = 8192, T: int = 100) -> Workload:
     return Workload(f"quadrotor_vanilla_N{N}_T{T}", "vanilla", dyn, cost, sampler, N, T, 1, 0.02, 1.0, 0.0, x0, U0)
 
 
+def quadrotor_gate_course() -> list:
+    """Three gates as waypoints (x, y, z, heading). The gate's corners lie along `heading` (QuadrotorMapCostParams::
+    updateWaypoint), so a gate crossed flying along +x has heading pi/2."""
+    return [(6.0, 0.0, 2.0, math.pi / 2), (12.0, 2.0, 2.5, math.pi / 2 - 0.3), (18.0, 3.0, 2.0, math.pi / 2)]
+
+
+def quadrotor_track_map(seed: int = 7, resolution: float = 0.25) -> tuple:
+    """A track cost map for quadrotor_gate_course(): 0.5 per metre of horizontal distance from the polyline through the
+    start and the gates, plus seeded noise in [0, 0.05). The map covers x in [-4, 24], y in [-8, 11]; outside it the cost's
+    map term adds crash_coeff. Returns (TwoDTextureHelper, x bounds, y bounds)."""
+    xb, yb = (-4.0, 24.0), (-8.0, 11.0)
+    w, h = int(round((xb[1] - xb[0]) / resolution)), int(round((yb[1] - yb[0]) / resolution))
+    pts = np.array([(0.0, 0.0)] + [g[:2] for g in quadrotor_gate_course()], np.float64)
+    cx = xb[0] + (np.arange(w) + 0.5) * resolution
+    cy = yb[0] + (np.arange(h) + 0.5) * resolution
+    X, Y = np.meshgrid(cx, cy)  # [h][w]
+    dist = np.full(X.shape, np.inf)
+    for a, b in zip(pts[:-1], pts[1:]):
+        ab = b - a
+        t = np.clip(((X - a[0]) * ab[0] + (Y - a[1]) * ab[1]) / (ab @ ab), 0.0, 1.0)
+        dist = np.minimum(dist, np.hypot(X - a[0] - t * ab[0], Y - a[1] - t * ab[1]))
+    values = (0.5 * dist + 0.05 * np.random.RandomState(seed).uniform(0.0, 1.0, dist.shape)).astype(np.float32)
+    tex = H.TwoDTextureHelper()
+    tex.setExtent(0, w, h)
+    tex.updateTexture(0, values)
+    tex.updateOrigin(0, (xb[0], yb[0], 0.0))
+    tex.updateResolution(0, resolution)
+    tex.enableTexture(0)
+    return tex, xb, yb
+
+
+def quadrotor_gates(N: int = 8192, T: int = 100, use_map: bool = True) -> Workload:
+    """Quadrotor + QuadrotorMapCost flying quadrotor_gate_course() over quadrotor_track_map() (without the map when
+    use_map is False), VanillaMPPI. The cost starts with the start point as its previous waypoint and the first gate as
+    its current one; advance_quadrotor_gate() moves to the next gate once the current one is passed. extra["gate"] is the
+    index of the current gate."""
+    w = quadrotor(N, T)
+    cost = H.QuadrotorMapCost()
+    cost.params.desired_speed = 3.0
+    cost.params.dist_to_waypoint_coeff = 1.0
+    start = (0.0, 0.0, 2.0, 0.0)
+    cost.updateWaypoint(start)
+    cost.updateWaypoint(quadrotor_gate_course()[0])
+    if use_map:
+        cost.tex_helper_ = quadrotor_track_map()[0]
+    w.cost = cost
+    w.x0[0, :3] = start[:3]
+    w.name = f"quadrotor_gates{'' if use_map else '_nomap'}_N{N}_T{T}"
+    w.extra = {"gate": 0, "start": start}
+    return w
+
+
+def advance_quadrotor_gate(w: Workload, state, radius: float = 1.0) -> bool:
+    """Move the cost's waypoint to the next gate once `state` is within `radius` of the current gate or past its plane
+    (the gate's plane contains the gate line and the vertical). Returns True if the waypoint moved."""
+    gates = quadrotor_gate_course()
+    g = w.extra["gate"]
+    if g >= len(gates) - 1:
+        return False
+    gx, gy, gz, hd = gates[g]
+    prev = w.extra["start"] if g == 0 else gates[g - 1]
+    nx, ny = -math.sin(hd), math.cos(hd)  # normal of the gate line
+    side = lambda x, y: (x - gx) * nx + (y - gy) * ny  # noqa: E731
+    passed = side(state[0], state[1]) * side(prev[0], prev[1]) < 0
+    if passed or math.dist(state[:3], (gx, gy, gz)) < radius:
+        w.extra["gate"] = g + 1
+        w.cost.updateWaypoint(gates[g + 1])
+        return True
+    return False
+
+
 BUILDERS = {
     "racer_lstm": racer_lstm,
     "racer_lstm_gaussian": racer_lstm_gaussian,
@@ -243,6 +314,7 @@ BUILDERS = {
     "autorally_robust": autorally_robust,
     "double_integrator_robust_tube": double_integrator_robust_tube,
     "quadrotor": quadrotor,
+    "quadrotor_gates": quadrotor_gates,
 }
 
 
