@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <type_traits>
 #include <mutex>
@@ -899,7 +900,8 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return fail(MPPIB_ERR_INVALID_ARG, "device %d out of range (%d devices)", desc->device, ndev);
   CUDA_TRY(cudaSetDevice(desc->device));
 
-  mppib_engine* e = new mppib_engine();
+  std::unique_ptr<mppib_engine> owner(new mppib_engine());  // every early return below releases what was made so far
+  mppib_engine* e = owner.get();
   e->desc = *desc;
   e->desc.world_size = world;
   e->S = entry->S;
@@ -921,10 +923,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   e->cost_shared_floats = entry->cost_shared_floats;
   e->rmppi = (desc->flags & MPPIB_FLAG_RMPPI) != 0;
   if (e->rmppi && desc->num_distributions != 2)
-  {
-    delete e;
     return fail(MPPIB_ERR_INVALID_ARG, "MPPIB_FLAG_RMPPI needs num_distributions == 2 (nominal, real)");
-  }
   e->writeback = e->rmppi || (desc->flags & MPPIB_FLAG_WRITEBACK_CONTROLS) != 0;
   e->use_pdl = !getenv("MPPIB_NO_PDL");
   e->mapped_result = !getenv("MPPIB_NO_MAPPED_RESULT");
@@ -932,49 +931,29 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   // MPPIB_SPIN_WAIT is set
   e->spin_wait = e->mapped_result && getenv("MPPIB_SPIN_WAIT") != nullptr;
 
-  auto bail = [&](int rc) {
-    mppib_destroy(e);
-    return rc;
-  };
-
   if (e->D * e->TC > kMaxMeanFloats)
-    return bail(fail(MPPIB_ERR_UNSUPPORTED, "D*T*C = %d exceeds %d", e->D * e->TC, kMaxMeanFloats));
+    return fail(MPPIB_ERR_UNSUPPORTED, "D*T*C = %d exceeds %d", e->D * e->TC, kMaxMeanFloats);
   e->nchunks = (e->TC + kChunkFloats - 1) / kChunkFloats;
   if (e->nchunks > kMaxChunks)
-    return bail(fail(MPPIB_ERR_UNSUPPORTED, "T*C = %d exceeds %d", e->TC, kMaxChunks * kChunkFloats));
+    return fail(MPPIB_ERR_UNSUPPORTED, "T*C = %d exceeds %d", e->TC, kMaxChunks * kChunkFloats);
 
   // rollout sharding (SURVEY §8e): contiguous slices, remainder to the last rank
   const int per = e->N / world;
   e->n_offset = per * desc->rank;
   e->n_local = (desc->rank == world - 1) ? (e->N - e->n_offset) : per;
   if (e->n_local <= 0)
-    return bail(fail(MPPIB_ERR_INVALID_ARG, "rank %d of %d has no rollouts (N=%d)", desc->rank, world, e->N));
+    return fail(MPPIB_ERR_INVALID_ARG, "rank %d of %d has no rollouts (N=%d)", desc->rank, world, e->N);
 
   if (int rc = choose_k1(e, entry, ov))
-    return bail(rc);
+    return rc;
   e->pstride = ((kPartialHeader + e->TC + 3) / 4) * 4;
 
+  int prio_lo = 0, prio_hi = 0;
+  CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
   if (desc->stream)
-    e->stream = (cudaStream_t)desc->stream;
+    e->stream.borrow((cudaStream_t)desc->stream);
   else
-  {
-    int prio_lo = 0, prio_hi = 0;
-    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    if (cudaStreamCreateWithPriority(&e->stream, cudaStreamNonBlocking, prio_hi) != cudaSuccess)
-      return bail(fail(MPPIB_ERR_CUDA, "cudaStreamCreate failed"));
-    e->own_stream = true;
-  }
-
-#define CUDA_TRY_B(expr)                                                                                               \
-  do                                                                                                                   \
-  {                                                                                                                    \
-    cudaError_t _e = (expr);                                                                                           \
-    if (_e != cudaSuccess)                                                                                             \
-    {                                                                                                                  \
-      cudaGetLastError();                                                                                              \
-      return bail(fail(MPPIB_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)));                               \
-    }                                                                                                                  \
-  } while (0)
+    CUDA_TRY(e->stream.create(cudaStreamNonBlocking, prio_hi));
 
   const size_t noise_floats = (size_t)e->n_local * e->TC;
   const size_t lead_floats = 8192;  // room for the offset-alignment lead-in (see draw_noise)
@@ -990,73 +969,63 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     e->draw_start = per_rollout * (unsigned long long)e->n_offset;
     e->draw_local = (size_t)(per_rollout * (unsigned long long)e->n_local);
   }
-  CUDA_TRY_B(cudaMalloc(&e->noise_alloc, (lead_floats + noise_floats + 8) * sizeof(float)));
+  CUDA_TRY(e->noise_alloc.alloc(lead_floats + noise_floats + 8));
   e->eps_d = e->noise_alloc + lead_floats;  // cudaMalloc is 256-B aligned and 8192*4 keeps that
-  CUDA_TRY_B(cudaMemsetAsync(e->noise_alloc, 0, (lead_floats + noise_floats + 8) * sizeof(float), e->stream));
+  CUDA_TRY(cudaMemsetAsync(e->noise_alloc, 0, (lead_floats + noise_floats + 8) * sizeof(float), e->stream));
   e->eps_buf[0] = e->eps_buf[1] = e->eps_d;
   e->prefetch_enabled = !(desc->flags & MPPIB_FLAG_NO_PREFETCH) && !getenv("MPPIB_NO_PREFETCH");
-  CUDA_TRY_B(cudaEventCreateWithFlags(&e->ev_last_gen, cudaEventDisableTiming));
+  CUDA_TRY(e->ev_last_gen.create(cudaEventDisableTiming));
   if (e->prefetch_enabled)
   {
-    CUDA_TRY_B(cudaMalloc(&e->noise_alloc2, (lead_floats + noise_floats + 8) * sizeof(float)));
-    CUDA_TRY_B(cudaMemsetAsync(e->noise_alloc2, 0, (lead_floats + noise_floats + 8) * sizeof(float), e->stream));
+    CUDA_TRY(e->noise_alloc2.alloc(lead_floats + noise_floats + 8));
+    CUDA_TRY(cudaMemsetAsync(e->noise_alloc2, 0, (lead_floats + noise_floats + 8) * sizeof(float), e->stream));
     e->eps_buf[1] = e->noise_alloc2 + lead_floats;
-    {
-      // the prefetch (next solve's noise) yields to the solve in flight: lowest priority for the side stream
-      int prio_lo = 0, prio_hi = 0;
-      CUDA_TRY_B(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-      CUDA_TRY_B(cudaStreamCreateWithPriority(&e->side_stream, cudaStreamNonBlocking, prio_lo));
-    }
+    // the prefetch (next solve's noise) yields to the solve in flight: lowest priority for the side stream
+    CUDA_TRY(e->side_stream.create(cudaStreamNonBlocking, prio_lo));
     for (int i = 0; i < 2; i++)
     {
-      CUDA_TRY_B(cudaEventCreateWithFlags(&e->ev_k1_done[i], cudaEventDisableTiming));
-      CUDA_TRY_B(cudaEventCreateWithFlags(&e->ev_gen_done[i], cudaEventDisableTiming));
+      CUDA_TRY(e->ev_k1_done[i].create(cudaEventDisableTiming));
+      CUDA_TRY(e->ev_gen_done[i].create(cudaEventDisableTiming));
     }
   }
-  CUDA_TRY_B(cudaMalloc(&e->costs_d, (size_t)e->D * e->n_local * sizeof(float)));
-  CUDA_TRY_B(cudaMalloc(&e->partials_d, (size_t)e->grid * e->D * e->pstride * sizeof(float)));
-  CUDA_TRY_B(cudaMalloc(&e->headers_d, (size_t)e->grid * e->D * sizeof(float4)));
-  CUDA_TRY_B(cudaMalloc(&e->result_d, (size_t)e->D * e->pstride * sizeof(float)));
-  CUDA_TRY_B(cudaHostAlloc(&e->result_h, (size_t)e->D * e->pstride * sizeof(float), cudaHostAllocMapped));
+  CUDA_TRY(e->costs_d.alloc((size_t)e->D * e->n_local));
+  CUDA_TRY(e->partials_d.alloc((size_t)e->grid * e->D * e->pstride));
+  CUDA_TRY(e->headers_d.alloc((size_t)e->grid * e->D));
+  CUDA_TRY(e->result_d.alloc((size_t)e->D * e->pstride));
+  CUDA_TRY(e->result_h.alloc((size_t)e->D * e->pstride, cudaHostAllocMapped, &e->result_h_dev));
   memset(e->result_h, 0, (size_t)e->D * e->pstride * sizeof(float));
-  CUDA_TRY_B(cudaHostGetDevicePointer(&e->result_h_dev, e->result_h, 0));
-  CUDA_TRY_B(cudaMalloc(&e->k2_counter_d, sizeof(unsigned)));
-  CUDA_TRY_B(cudaMemsetAsync(e->k2_counter_d, 0, sizeof(unsigned), e->stream));
-  {
-    unsigned* f = nullptr;
-    CUDA_TRY_B(cudaHostAlloc(&f, 64, cudaHostAllocMapped));
-    *f = 0u;
-    e->done_flag_h = f;
-    CUDA_TRY_B(cudaHostGetDevicePointer(&e->done_flag_dev, f, 0));
-  }
+  CUDA_TRY(e->k2_counter_d.alloc(1));
+  CUDA_TRY(cudaMemsetAsync(e->k2_counter_d, 0, sizeof(unsigned), e->stream));
+  CUDA_TRY(e->done_flag_h.alloc(16, cudaHostAllocMapped, &e->done_flag_dev));  // 64 bytes
+  *e->done_flag_h = 0u;
   if (e->writeback)
-    CUDA_TRY_B(cudaMalloc(&e->controls_d, (size_t)e->D * noise_floats * sizeof(float)));
+    CUDA_TRY(e->controls_d.alloc((size_t)e->D * noise_floats));
   if (world > 1)
   {
-    CUDA_TRY_B(cudaMalloc(&e->rank_rec_d, (size_t)e->D * e->pstride * sizeof(float)));
-    CUDA_TRY_B(cudaMalloc(&e->gather_d, (size_t)world * e->D * e->pstride * sizeof(float)));
-    CUDA_TRY_B(cudaMalloc(&e->gather_hdr_d, (size_t)world * e->D * sizeof(float4)));
+    CUDA_TRY(e->rank_rec_d.alloc((size_t)e->D * e->pstride));
+    CUDA_TRY(e->gather_d.alloc((size_t)world * e->D * e->pstride));
+    CUDA_TRY(e->gather_hdr_d.alloc((size_t)world * e->D));
   }
   for (int i = 0; i < 4; i++)
-    CUDA_TRY_B(cudaEventCreate(&e->ev[i]));
+    CUDA_TRY(e->ev[i].create());
 
   if (e->nln)
-    CUDA_TRY_B(cudaMalloc(&e->nln_d, noise_floats * sizeof(float)));
+    CUDA_TRY(e->nln_d.alloc(noise_floats));
   if (e->colored)
   {
     // spectrum (the raw draw), time-domain buffer, tables and the reference's plan (colored_noise.cu:236-282)
     const size_t batch = (size_t)e->n_local * e->C;
-    CUDA_TRY_B(cudaMalloc(&e->spec_alloc, (lead_floats + e->draw_local + 8) * sizeof(float)));
-    CUDA_TRY_B(cudaMemsetAsync(e->spec_alloc, 0, (lead_floats + e->draw_local + 8) * sizeof(float), e->stream));
+    CUDA_TRY(e->spec_alloc.alloc(lead_floats + e->draw_local + 8));
+    CUDA_TRY(cudaMemsetAsync(e->spec_alloc, 0, (lead_floats + e->draw_local + 8) * sizeof(float), e->stream));
     e->spec_d = reinterpret_cast<float2*>(e->spec_alloc + lead_floats);
-    CUDA_TRY_B(cudaMalloc(&e->time_d, batch * 2 * e->T * sizeof(float)));
-    CUDA_TRY_B(cudaMalloc(&e->coeffs_d, (size_t)e->C * e->F * sizeof(float)));
-    CUDA_TRY_B(cudaMalloc(&e->sigma_d, (size_t)e->C * sizeof(float)));
-    CUDA_TRY_B(cudaMalloc(&e->decay_pow_d, (size_t)e->T * sizeof(float)));
-    CUDA_TRY_B(cudaEventCreateWithFlags(&e->ev_rearr, cudaEventDisableTiming));
+    CUDA_TRY(e->time_d.alloc(batch * 2 * e->T));
+    CUDA_TRY(e->coeffs_d.alloc((size_t)e->C * e->F));
+    CUDA_TRY(e->sigma_d.alloc((size_t)e->C));
+    CUDA_TRY(e->decay_pow_d.alloc((size_t)e->T));
+    CUDA_TRY(e->ev_rearr.create(cudaEventDisableTiming));
     const cufftResult fr = cufftPlan1d(&e->fft_plan, 2 * e->T, CUFFT_C2R, (int)batch);
     if (fr != CUFFT_SUCCESS)
-      return bail(fail(MPPIB_ERR_CUDA, "cufftPlan1d(%d, C2R, %zu) failed: %d", 2 * e->T, batch, (int)fr));
+      return fail(MPPIB_ERR_CUDA, "cufftPlan1d(%d, C2R, %zu) failed: %d", 2 * e->T, batch, (int)fr);
     e->have_plan = true;
   }
 
@@ -1085,11 +1054,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     xorwow_nibble_tables(XorwowMatrix::power(jump_draws), tables);
     e->xw_jump_d = (uint32_t)(kXorwowWeyl * (uint32_t)(jump_draws & 0xffffffffULL));
     const size_t nstates = (size_t)K * kXorwowStreams;
-    CUDA_TRY_B(cudaMalloc(&e->xw_states_d, nstates * 6 * sizeof(uint32_t)));
-    CUDA_TRY_B(cudaMalloc(&e->xw_tables_d, tables.size() * sizeof(uint32_t)));
-    CUDA_TRY_B(cudaMemcpyAsync(e->xw_tables_d, tables.data(), tables.size() * sizeof(uint32_t), cudaMemcpyHostToDevice,
+    CUDA_TRY(e->xw_states_d.alloc(nstates * 6));
+    CUDA_TRY(e->xw_tables_d.alloc(tables.size()));
+    CUDA_TRY(cudaMemcpyAsync(e->xw_tables_d, tables.data(), tables.size() * sizeof(uint32_t), cudaMemcpyHostToDevice,
                                e->stream));
-    CUDA_TRY_B(cudaStreamSynchronize(e->stream));
+    CUDA_TRY(cudaStreamSynchronize(e->stream));
     e->xw_enabled = true;
     if (getenv("MPPIB_DEBUG"))
       fprintf(stderr, "[mppib] create: engine %p states %p tables %p (%zu B)\n", (void*)e, (void*)e->xw_states_d,
@@ -1099,33 +1068,41 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (e->use_tma)
   {
     for (int i = 0; i < 2; i++)
-    {
-      int rc = make_tensor_map(*e, e->eps_buf[i], &e->tmap_buf[i]);
-      if (rc != MPPIB_OK)
-        return bail(rc);
-    }
+      if (int rc = make_tensor_map(*e, e->eps_buf[i], &e->tmap_buf[i]))
+        return rc;
     e->tmap = e->tmap_buf[0];
   }
-  {
-    int rc = e->prepare(*e);
-    if (rc != MPPIB_OK)
-      return bail(rc);
-  }
+  if (int rc = e->prepare(*e))
+    return rc;
 
   // Controller::createAndSeedCUDARandomNumberGen (controller.cu:192-207): XORWOW, seed, offset 0
-  if (curandCreateGenerator(&e->gen, CURAND_RNG_PSEUDO_DEFAULT) != CURAND_STATUS_SUCCESS)
-    return bail(fail(MPPIB_ERR_CURAND, "curandCreateGenerator failed"));
-  if (curandSetStream(e->gen, e->stream) != CURAND_STATUS_SUCCESS)
-    return bail(fail(MPPIB_ERR_CURAND, "curandSetStream failed"));
-  {
-    int rc = mppib_seed(e, 0ULL, 0ULL);
-    if (rc != MPPIB_OK)
-      return bail(rc);
-  }
-  CUDA_TRY_B(cudaStreamSynchronize(e->stream));
-#undef CUDA_TRY_B
-  *out = e;
+  CURAND_TRY(curandCreateGenerator(&e->gen, CURAND_RNG_PSEUDO_DEFAULT));
+  CURAND_TRY(curandSetStream(e->gen, e->stream));
+  if (int rc = mppib_seed(e, 0ULL, 0ULL))
+    return rc;
+  CUDA_TRY(cudaStreamSynchronize(e->stream));
+  *out = owner.release();
   return MPPIB_OK;
+}
+
+// What must go before the members release themselves: both streams drained, then what hangs on them. The members follow in
+// reverse order of declaration, the streams last (engine_internal.cuh).
+mppib_engine::~mppib_engine()
+{
+  cudaSetDevice(desc.device);
+  if (side_stream)
+    cudaStreamSynchronize(side_stream);
+  if (stream)
+    cudaStreamSynchronize(stream);
+  if (comm && g_nccl.CommDestroy)
+    g_nccl.CommDestroy(comm);
+  for (int r = 0; r < 8; r++)
+    if (peer_opened[r])
+      cudaIpcCloseMemHandle(peer_opened[r]);
+  if (gen)
+    curandDestroyGenerator(gen);
+  if (have_plan)
+    cufftDestroy(fft_plan);
 }
 
 int mppib_destroy(mppib_engine* e)
@@ -1134,97 +1111,16 @@ int mppib_destroy(mppib_engine* e)
     return MPPIB_OK;
   if (getenv("MPPIB_DEBUG"))
     fprintf(stderr, "[mppib] destroy: engine %p\n", (void*)e);
-  cudaSetDevice(e->desc.device);
-  if (e->side_stream)
-    cudaStreamSynchronize(e->side_stream);
-  if (e->stream)
-    cudaStreamSynchronize(e->stream);
-  if (e->comm && g_nccl.CommDestroy)
-    g_nccl.CommDestroy(e->comm);
-  for (int r = 0; r < 8; r++)
-    if (e->peer_opened[r])
-      cudaIpcCloseMemHandle(e->peer_opened[r]);
-  cudaFree(e->p2p_gather_d);
-  if (e->gen)
-    curandDestroyGenerator(e->gen);
-  if (e->costmap_tex)
-    cudaDestroyTextureObject(e->costmap_tex);
-  if (e->costmap_array)
-    cudaFreeArray(e->costmap_array);
-  cudaFree(e->nn_theta_d);
-  cudaFree(e->lstm_theta_d);
-  cudaFree(e->elev_d);
-  cudaFree(e->cost_tex_d);
-  cudaFree(e->fb_gains_d);
-  cudaFree(e->ddp_ws_d);
-  cudaFree(e->ddp_status_d);
-  cudaFree(e->eval_states_d);
-  cudaFree(e->eval_strides_d);
-  cudaFree(e->eval_costs_d);
-  cudaFree(e->nln_d);
-  cudaFree(e->vis_idx_d);
-  cudaFree(e->vis_opt_d);
-  cudaFree(e->nom_d);
-  cudaFree(e->nom_u_d);
-  if (e->nom_h)
-    cudaFreeHost(e->nom_h);
-  cudaFree(e->vis_outputs_d);
-  cudaFree(e->vis_costs_d);
-  cudaFree(e->vis_crash_d);
-  cudaFree(e->noise_alloc);
-  cudaFree(e->noise_alloc2);
-  cudaFree(e->costs_d);
-  cudaFree(e->partials_d);
-  cudaFree(e->headers_d);
-  cudaFree(e->gather_hdr_d);
-  cudaFree(e->controls_d);
-  cudaFree(e->rank_rec_d);
-  cudaFree(e->gather_d);
-  cudaFree(e->result_d);
-  cudaFree(e->weights_d);
-  cudaFree(e->l2_flush_d);
-  cudaFree(e->xw_states_d);
-  cudaFree(e->xw_tables_d);
-  if (e->have_plan)
-    cufftDestroy(e->fft_plan);
-  cudaFree(e->spec_alloc);
-  cudaFree(e->time_d);
-  cudaFree(e->coeffs_d);
-  cudaFree(e->sigma_d);
-  cudaFree(e->decay_pow_d);
-  if (e->ev_rearr)
-    cudaEventDestroy(e->ev_rearr);
-  if (e->result_h)
-    cudaFreeHost(e->result_h);
-  if (e->done_flag_h)
-    cudaFreeHost((void*)e->done_flag_h);
-  cudaFree(e->k2_counter_d);
-  for (int i = 0; i < 4; i++)
-    if (e->ev[i])
-      cudaEventDestroy(e->ev[i]);
-  for (int i = 0; i < 2; i++)
-  {
-    if (e->ev_k1_done[i])
-      cudaEventDestroy(e->ev_k1_done[i]);
-    if (e->ev_gen_done[i])
-      cudaEventDestroy(e->ev_gen_done[i]);
-  }
-  if (e->ev_last_gen)
-    cudaEventDestroy(e->ev_last_gen);
-  if (e->side_stream)
-    cudaStreamDestroy(e->side_stream);
-  if (e->own_stream && e->stream)
-    cudaStreamDestroy(e->stream);
-  cudaGetLastError();
   delete e;
+  cudaGetLastError();
   return MPPIB_OK;
 }
 
 // A TwoDTextureHelper<float> map in the mppib_elevation_map_header + row-major floats format (params.h): validates the
 // header, grows the device buffer when needed and copies the values. Used by both map blobs (the RACER models' elevation
 // map and QuadrotorMapCost's costmap); `what` names the blob in the error text.
-static int upload_map_blob(mppib_engine& e, const char* what, const void* host, size_t nbytes, float*& data_d,
-                           size_t& capacity, mppib_elevation_map_header& hdr)
+static int upload_map_blob(mppib_engine& e, const char* what, const void* host, size_t nbytes, DeviceBuffer<float>& data_d,
+                           mppib_elevation_map_header& hdr)
 {
   if (nbytes < sizeof(mppib_elevation_map_header))
     return fail(MPPIB_ERR_INVALID_ARG, "%s: %zu bytes is smaller than its header", what, nbytes);
@@ -1242,15 +1138,7 @@ static int upload_map_blob(mppib_engine& e, const char* what, const void* host, 
   for (int i = 0; i < 9; i++)
     if (!std::isfinite(h.rotations[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "%s: rotation entry %d is not finite", what, i);
-  if (cells > capacity)
-  {
-    CUDA_TRY(cudaStreamSynchronize(e.stream));
-    cudaFree(data_d);
-    data_d = nullptr;
-    capacity = 0;
-    CUDA_TRY(cudaMalloc(&data_d, cells * sizeof(float)));
-    capacity = cells;
-  }
+  CUDA_TRY(data_d.reserve(cells, e.stream));
   CUDA_TRY(cudaMemcpyAsync(data_d, (const char*)host + sizeof(h), cells * sizeof(float), cudaMemcpyHostToDevice, e.stream));
   CUDA_TRY(cudaStreamSynchronize(e.stream));
   hdr = h;
@@ -1360,7 +1248,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
         if (!std::isfinite(w[i]))  // fnn_helper.cu:244-247 asserts finiteness
           return fail(MPPIB_ERR_INVALID_ARG, "NN weight %d is not finite", i);
       if (!e->nn_theta_d)
-        CUDA_TRY(cudaMalloc(&e->nn_theta_d, nbytes));
+        CUDA_TRY(e->nn_theta_d.alloc(MPPIB_AR_NN_NUM_PARAMS));
       CUDA_TRY(cudaMemcpyAsync(e->nn_theta_d, host, nbytes, cudaMemcpyHostToDevice, e->stream));
       CUDA_TRY(cudaStreamSynchronize(e->stream));
       e->nn_theta_h.assign(w, w + MPPIB_AR_NN_NUM_PARAMS);
@@ -1380,7 +1268,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
         if (!std::isfinite(w[i]))
           return fail(MPPIB_ERR_INVALID_ARG, "LSTM weight %zu is not finite", i);
       if (!e->lstm_theta_d)
-        CUDA_TRY(cudaMalloc(&e->lstm_theta_d, nbytes));
+        CUDA_TRY(e->lstm_theta_d.alloc(nbytes / sizeof(float)));
       CUDA_TRY(cudaMemcpyAsync(e->lstm_theta_d, host, nbytes, cudaMemcpyHostToDevice, e->stream));
       CUDA_TRY(cudaStreamSynchronize(e->stream));
       e->lstm_theta_h.assign(w, w + nbytes / sizeof(float));
@@ -1394,7 +1282,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
       if (e->desc.dynamics_id != MPPIB_DYN_RACER_LSTM)
         return fail(MPPIB_ERR_INVALID_ARG, "elevation map given to a dynamics without one");
       // the values themselves may be NaN (unobserved cells): the model's own isfinite guards handle that (racer_dubins.cu:414-425)
-      const int rc = upload_map_blob(*e, "elevation map", host, nbytes, e->elev_d, e->elev_capacity, e->elev_hdr);
+      const int rc = upload_map_blob(*e, "elevation map", host, nbytes, e->elev_d, e->elev_hdr);
       if (rc != MPPIB_OK)
         return rc;
       e->elev_h.assign((const unsigned char*)host, (const unsigned char*)host + nbytes);
@@ -1404,7 +1292,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
       // QuadrotorMapCost's tex_helper_ map 0 (quadrotor_map_cost.cu:37-61), the same format
       if (e->desc.cost_id != MPPIB_COST_QUADROTOR_MAP)
         return fail(MPPIB_ERR_INVALID_ARG, "cost texture given to a cost without one");
-      return upload_map_blob(*e, "cost texture", host, nbytes, e->cost_tex_d, e->cost_tex_capacity, e->cost_tex_hdr);
+      return upload_map_blob(*e, "cost texture", host, nbytes, e->cost_tex_d, e->cost_tex_hdr);
     case MPPIB_BLOB_COSTMAP:
     {
       if (!cost_has_map(e->desc.cost_id))
@@ -1417,26 +1305,8 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
       if (cp.map_width <= 0 || cp.map_height <= 0 || nbytes != expect)
         return fail(MPPIB_ERR_INVALID_ARG, "costmap: got %zu bytes, expected %zu (%d x %d float4)", nbytes, expect,
                     cp.map_width, cp.map_height);
-      if (e->costmap_tex)
-      {
-        cudaDestroyTextureObject(e->costmap_tex);
-        e->costmap_tex = 0;
-      }
-      if (e->costmap_array)
-      {
-        cudaFreeArray(e->costmap_array);
-        e->costmap_array = nullptr;
-      }
       // ar_standard_cost.cu:101-176: float4 array, clamp, point filter, element read, normalised coordinates
       cudaChannelFormatDesc ch = cudaCreateChannelDesc(32, 32, 32, 32, cudaChannelFormatKindFloat);
-      CUDA_TRY(cudaMallocArray(&e->costmap_array, &ch, cp.map_width, cp.map_height));
-      CUDA_TRY(cudaMemcpy2DToArrayAsync(e->costmap_array, 0, 0, host, (size_t)cp.map_width * 16,
-                                        (size_t)cp.map_width * 16, cp.map_height, cudaMemcpyHostToDevice, e->stream));
-      CUDA_TRY(cudaStreamSynchronize(e->stream));
-      cudaResourceDesc res;
-      memset(&res, 0, sizeof(res));
-      res.resType = cudaResourceTypeArray;
-      res.res.array.array = e->costmap_array;
       cudaTextureDesc tex;
       memset(&tex, 0, sizeof(tex));
       tex.addressMode[0] = cudaAddressModeClamp;
@@ -1444,7 +1314,7 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
       tex.filterMode = cudaFilterModePoint;
       tex.readMode = cudaReadModeElementType;
       tex.normalizedCoords = 1;
-      CUDA_TRY(cudaCreateTextureObject(&e->costmap_tex, &res, &tex, nullptr));
+      CUDA_TRY(e->costmap_tex.replace(ch, cp.map_width, cp.map_height, host, (size_t)cp.map_width * 16, tex, e->stream));
       return MPPIB_OK;
     }
     default:
@@ -1543,7 +1413,7 @@ int mppib_comm_p2p_handle(mppib_engine* e, void* handle_64)
   if (!e->p2p_gather_d)
   {
     const size_t floats = (size_t)2 * world * e->D * e->pstride + 2 * world + 16;
-    CUDA_TRY(cudaMalloc(&e->p2p_gather_d, floats * sizeof(float)));
+    CUDA_TRY(e->p2p_gather_d.alloc(floats));
     CUDA_TRY(cudaMemset(e->p2p_gather_d, 0, floats * sizeof(float)));
   }
   cudaIpcMemHandle_t h;
@@ -1654,7 +1524,7 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
   if (rc != MPPIB_OK)
     return rc;
   if (e->l2_flush_d)
-    CUDA_TRY(cudaMemsetAsync(e->l2_flush_d, 0, e->l2_flush_bytes, e->stream));
+    CUDA_TRY(cudaMemsetAsync(e->l2_flush_d, 0, e->l2_flush_d.capacity(), e->stream));
   if (e->timing)
     CUDA_TRY(cudaEventRecord(e->ev[1], e->stream));
   rc = e->launch_rollout(*e, x0, U_in, optimization_stride, iteration_num);
@@ -1851,15 +1721,14 @@ int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* fe
       if (!std::isfinite(feedback_gains[i]))
         return fail(MPPIB_ERR_INVALID_ARG, "feedback gain %zu is not finite", i);
     if (!e->fb_gains_d)
-      CUDA_TRY(cudaMalloc(&e->fb_gains_d, n * sizeof(float)));
+      CUDA_TRY(e->fb_gains_d.alloc(n));
     CUDA_TRY(cudaMemcpyAsync(e->fb_gains_d, feedback_gains, n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     CUDA_TRY(cudaStreamSynchronize(e->stream));
   }
   else if (e->fb_gains_d)
   {
     CUDA_TRY(cudaStreamSynchronize(e->stream));
-    cudaFree(e->fb_gains_d);
-    e->fb_gains_d = nullptr;
+    e->fb_gains_d.reset();
   }
   return MPPIB_OK;
 }
@@ -1915,20 +1784,12 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
     if (!std::isfinite(u_target[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "u_target entry %zu is not finite", i);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  if (T > e->ddp_capacity)
-  {
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    cudaFree(e->ddp_ws_d);
-    e->ddp_ws_d = nullptr;
-    e->ddp_capacity = 0;
-    CUDA_TRY(cudaMalloc(&e->ddp_ws_d, ddp::ws_layout(T, S, C).total * sizeof(float)));
-    e->ddp_capacity = T;
-  }
+  CUDA_TRY(e->ddp_ws_d.reserve(ddp::ws_layout(T, S, C).total, e->stream));
   if (!e->ddp_status_d)
-    CUDA_TRY(cudaMalloc(&e->ddp_status_d, sizeof(int)));
+    CUDA_TRY(e->ddp_status_d.alloc(1));
   if (to_rmppi && !e->fb_gains_d)
   {
-    CUDA_TRY(cudaMalloc(&e->fb_gains_d, (size_t)T * S * C * sizeof(float)));
+    CUDA_TRY(e->fb_gains_d.alloc((size_t)T * S * C));
     CUDA_TRY(cudaMemsetAsync(e->fb_gains_d, 0, (size_t)T * S * C * sizeof(float), e->stream));
   }
   const ddp::WsLayout L = ddp::ws_layout(T, S, C);
@@ -1937,7 +1798,7 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
   CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
   // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
   CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  int rc = e->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d : nullptr);
+  int rc = e->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d.get() : nullptr);
   if (rc != MPPIB_OK)
     return rc;
   int status = 0;
@@ -1974,19 +1835,9 @@ int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides
     return fail(MPPIB_ERR_INVALID_ARG, "(number of candidates) * (samples per candidate) cannot exceed NUM_ROLLOUTS");
   CUDA_TRY(cudaSetDevice(e->desc.device));
   const int total = num_candidates * samples_per_candidate;
-  if (total > e->eval_capacity || !e->eval_states_d)
-  {
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    cudaFree(e->eval_states_d);
-    cudaFree(e->eval_strides_d);
-    cudaFree(e->eval_costs_d);
-    e->eval_states_d = nullptr;
-    e->eval_capacity = 0;
-    CUDA_TRY(cudaMalloc(&e->eval_states_d, (size_t)total * e->S * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&e->eval_strides_d, (size_t)total * sizeof(int)));
-    CUDA_TRY(cudaMalloc(&e->eval_costs_d, (size_t)total * sizeof(float)));
-    e->eval_capacity = total;
-  }
+  CUDA_TRY(e->eval_states_d.reserve((size_t)total * e->S, e->stream));
+  CUDA_TRY(e->eval_strides_d.reserve((size_t)total, e->stream));
+  CUDA_TRY(e->eval_costs_d.reserve((size_t)total, e->stream));
   CUDA_TRY(cudaMemcpyAsync(e->eval_states_d, candidates, (size_t)num_candidates * e->S * sizeof(float),
                            cudaMemcpyHostToDevice, e->stream));
   CUDA_TRY(cudaMemcpyAsync(e->eval_strides_d, strides, (size_t)num_candidates * sizeof(int), cudaMemcpyHostToDevice,
@@ -2040,25 +1891,12 @@ int mppib_sample_trajectories(mppib_engine* e, const float* x0, const float* U_n
     if (!std::isfinite(x0[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "x0[%d] is not finite", i);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  if (n > e->vis_capacity)
-  {
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    cudaFree(e->vis_idx_d);
-    cudaFree(e->vis_outputs_d);
-    cudaFree(e->vis_costs_d);
-    cudaFree(e->vis_crash_d);
-    e->vis_idx_d = nullptr;
-    e->vis_outputs_d = e->vis_costs_d = nullptr;
-    e->vis_crash_d = nullptr;
-    e->vis_capacity = 0;
-    CUDA_TRY(cudaMalloc(&e->vis_idx_d, (size_t)n * sizeof(int)));
-    CUDA_TRY(cudaMalloc(&e->vis_outputs_d, (size_t)n * e->T * e->O * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&e->vis_costs_d, (size_t)n * (e->T + 1) * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&e->vis_crash_d, (size_t)n * e->T * sizeof(int)));
-    e->vis_capacity = n;
-  }
+  CUDA_TRY(e->vis_idx_d.reserve((size_t)n, e->stream));
+  CUDA_TRY(e->vis_outputs_d.reserve((size_t)n * e->T * e->O, e->stream));
+  CUDA_TRY(e->vis_costs_d.reserve((size_t)n * (e->T + 1), e->stream));
+  CUDA_TRY(e->vis_crash_d.reserve((size_t)n * e->T, e->stream));
   if (have_opt && !e->vis_opt_d)
-    CUDA_TRY(cudaMalloc(&e->vis_opt_d, (size_t)e->TC * sizeof(float)));
+    CUDA_TRY(e->vis_opt_d.alloc((size_t)e->TC));
   CUDA_TRY(cudaMemcpyAsync(e->vis_idx_d, sample_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, e->stream));
   if (have_opt)
     CUDA_TRY(cudaMemcpyAsync(e->vis_opt_d, U_opt, (size_t)e->TC * sizeof(float), cudaMemcpyHostToDevice, e->stream));
@@ -2093,16 +1931,15 @@ int mppib_nominal_trajectory(mppib_engine* e, const float* x0, const float* U, c
   CUDA_TRY(cudaSetDevice(e->desc.device));
   const size_t n_u = (size_t)e->D * e->TC, n_s = (size_t)e->D * e->T * e->S, n_o = (size_t)e->D * e->T * e->O;
   if (!e->nom_d)
-  {
-    CUDA_TRY(cudaMalloc(&e->nom_d, (n_u + n_s + n_o) * sizeof(float)));
-    CUDA_TRY(cudaHostAlloc(&e->nom_h, (n_u + n_s + n_o) * sizeof(float), cudaHostAllocDefault));
-  }
+    CUDA_TRY(e->nom_d.alloc(n_u + n_s + n_o));
+  if (!e->nom_h)
+    CUDA_TRY(e->nom_h.alloc(n_u + n_s + n_o, cudaHostAllocDefault));
   const float* u_src = e->result_d + kPartialHeader;  // the optimised sequence where K2 / KX left it
   int u_stride = e->pstride;
   if (U)
   {
     if (!e->nom_u_d)
-      CUDA_TRY(cudaMalloc(&e->nom_u_d, n_u * sizeof(float)));
+      CUDA_TRY(e->nom_u_d.alloc(n_u));
     CUDA_TRY(cudaMemcpyAsync(e->nom_u_d, U, n_u * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     u_src = e->nom_u_d;
     u_stride = e->TC;
@@ -2144,17 +1981,9 @@ int mppib_set_option(mppib_engine* e, int option, long long value)
   {
     case MPPIB_OPT_L2_FLUSH_BYTES:
       CUDA_TRY(cudaStreamSynchronize(e->stream));
-      if (e->l2_flush_d)
-      {
-        cudaFree(e->l2_flush_d);
-        e->l2_flush_d = nullptr;
-        e->l2_flush_bytes = 0;
-      }
-      if (value > 0)
-      {
-        CUDA_TRY(cudaMalloc(&e->l2_flush_d, (size_t)value));
-        e->l2_flush_bytes = (size_t)value;
-      }
+      e->l2_flush_d.reset();
+      if (value > 0)  // exactly that many bytes: a larger buffer would change what is flushed
+        CUDA_TRY(e->l2_flush_d.alloc((size_t)value));
       return MPPIB_OK;
   }
   return fail(MPPIB_ERR_INVALID_ARG, "unknown option %d", option);
@@ -2204,7 +2033,7 @@ int mppib_get_weights(mppib_engine* e, float* host_weights)
   CUDA_TRY(cudaSetDevice(e->desc.device));
   const size_t n = (size_t)e->D * e->n_local;
   if (!e->weights_d)
-    CUDA_TRY(cudaMalloc(&e->weights_d, n * sizeof(float)));
+    CUDA_TRY(e->weights_d.alloc(n));
   const dim3 grid((e->n_local + 255) / 256 > 1024 ? 1024 : (e->n_local + 255) / 256, e->D);
   weights_kernel<<<grid, 256, 0, e->stream>>>(e->costs_d, e->result_d, e->n_local, e->pstride,
                                               (float)(1.0 / e->lambda), e->weights_d);

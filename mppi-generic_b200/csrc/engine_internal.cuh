@@ -27,6 +27,7 @@
 #include "../../include/mppi_b200.h"
 #include "combine_kernel.cuh"
 #include "ddp_kernel.cuh"
+#include "device_resources.cuh"
 #include "plugins/costs.cuh"
 #include "plugins/dynamics.cuh"
 #include "rollout_kernel.cuh"
@@ -63,8 +64,15 @@ typedef struct ncclComm* ncclComm_t;
 using namespace mppib;
 
 // ---- engine state -----------------------------------------------------------------------------------------------
+// Every device resource is a member that releases itself (device_resources.cuh); a buffer that grows does so through
+// reserve(). ~mppib_engine (engine.cu) drains the streams and releases what must go before them; the members follow.
 struct mppib_engine
 {
+  ~mppib_engine();
+  // the streams come before every buffer and event, so that they are destroyed after them
+  Stream stream;       // the solve's stream: the engine's own, or mppib_desc.stream borrowed
+  Stream side_stream;  // noise prefetch (null when prefetch is off)
+
   mppib_desc desc{};
   int S = 0, C = 0, O = 0, D = 1;
   int N = 0, T = 0, TC = 0;
@@ -87,43 +95,38 @@ struct mppib_engine
   int ws_pspw = 16;    // its samples per producer warp: threads per CTA = bx * (32 / ws_pspw + 1)
   bool mapped_result = true;  // K2 writes the result record straight into mapped pinned host memory
   bool spin_wait = true;      // the host waits for the solve by polling a mapped flag K2's last block sets
-  unsigned* k2_counter_d = nullptr;
-  volatile unsigned* done_flag_h = nullptr;
-  unsigned* done_flag_dev = nullptr;
+  DeviceBuffer<unsigned> k2_counter_d;
+  PinnedBuffer<volatile unsigned> done_flag_h;
+  volatile unsigned* done_flag_dev = nullptr;  // device alias of done_flag_h
   unsigned solve_seq = 0;
   bool flag_armed = false;  // the LAST enqueued solve ends in a kernel that publishes done_flag == solve_seq
   bool writeback = false;
   bool rmppi = false;  // MPPIB_FLAG_RMPPI
   float tsallis_gamma = 0.0f, tsallis_r = 0.0f;  // both non-zero: Tsallis weights (mppib_set_tsallis)
   float value_func_threshold = 1000.0f;  // robust_mppi_controller.cuh default
-  float* fb_gains_d = nullptr;           // [T][S][C] or null
-  float* eval_states_d = nullptr;        // init-eval scratch: candidates, strides, costs
-  int* eval_strides_d = nullptr;
-  float* eval_costs_d = nullptr;
-  int eval_capacity = 0;
+  DeviceBuffer<float> fb_gains_d;        // [T][S][C] or null
+  DeviceBuffer<float> eval_states_d;     // init-eval scratch: candidates, strides, costs
+  DeviceBuffer<int> eval_strides_d;
+  DeviceBuffer<float> eval_costs_d;
   int (*init_eval)(mppib_engine&, const float*, const int*, int, int, const float*, int) = nullptr;
   // sampled (visualisation) trajectories scratch: picked indices, optimised sequence, outputs / costs / crash flags
-  int* vis_idx_d = nullptr;
-  float* vis_opt_d = nullptr;
-  float* nom_d = nullptr;      // device tail: [D][T][C] smoothed controls | [D][T][S] states | [D][T][O] outputs
-  float* nom_h = nullptr;      // pinned host copy of the same
-  float* nom_u_d = nullptr;    // uploaded [D][T][C] when the caller passes its own U
+  DeviceBuffer<int> vis_idx_d;
+  DeviceBuffer<float> vis_opt_d;
+  DeviceBuffer<float> nom_d;    // device tail: [D][T][C] smoothed controls | [D][T][S] states | [D][T][O] outputs
+  PinnedBuffer<float> nom_h;    // pinned host copy of the same
+  DeviceBuffer<float> nom_u_d;  // uploaded [D][T][C] when the caller passes its own U
   int (*nominal_traj)(mppib_engine&, const float*, const float*, int, const float*) = nullptr;
-  float* vis_outputs_d = nullptr;
-  float* vis_costs_d = nullptr;
-  int* vis_crash_d = nullptr;
-  int vis_capacity = 0;
+  DeviceBuffer<float> vis_outputs_d;
+  DeviceBuffer<float> vis_costs_d;
+  DeviceBuffer<int> vis_crash_d;
   int (*sampled_traj)(mppib_engine&, const float*, const float*, int, int, bool) = nullptr;
   // DDP feedback (ddp_kernel.cuh, mppib_set_ddp / mppib_ddp_feedback): weights (empty = identity, DDPParams defaults), the
-  // workspace sized for ddp_capacity steps, the solve's status word, and the pair's launcher (null: no analytic Jacobian)
+  // workspace for the longest horizon so far, the solve's status word, and the pair's launcher (null: no analytic Jacobian)
   std::vector<float> ddp_Q, ddp_Qf, ddp_R;
   int ddp_iters = 1;
-  float* ddp_ws_d = nullptr;
-  int* ddp_status_d = nullptr;
-  int ddp_capacity = 0;
+  DeviceBuffer<float> ddp_ws_d;
+  DeviceBuffer<int> ddp_status_d;
   int (*ddp)(mppib_engine&, int T, const float* x0, float* gains_d) = nullptr;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
 
   // solver scalars
   float dt = 0.01f, lambda = 1.0f, alpha = 0.0f;
@@ -134,20 +137,17 @@ struct mppib_engine
   bool have_dyn = false, have_cost = false, have_sampler = false;
 
   // aux device resources
-  float* nn_theta_d = nullptr;
-  float* lstm_theta_d = nullptr;  // MPPIB_BLOB_LSTM_WEIGHTS
+  DeviceBuffer<float> nn_theta_d;
+  DeviceBuffer<float> lstm_theta_d;  // MPPIB_BLOB_LSTM_WEIGHTS
   bool have_lstm = false;
-  float* elev_d = nullptr;               // MPPIB_BLOB_ELEVATION_MAP: width * height floats, row-major
+  DeviceBuffer<float> elev_d;            // MPPIB_BLOB_ELEVATION_MAP: width * height floats, row-major
   // host copies of the weight / map blobs for mppib_compute_control's host tail (the library's host twins)
   std::vector<float> nn_theta_h, lstm_theta_h;
   std::vector<unsigned char> elev_h;
-  size_t elev_capacity = 0;              // floats allocated
   mppib_elevation_map_header elev_hdr{};  // use == 0 until a map is set
-  float* cost_tex_d = nullptr;               // MPPIB_BLOB_COST_TEXTURE: QuadrotorMapCost's map, width * height floats
-  size_t cost_tex_capacity = 0;              // floats allocated
+  DeviceBuffer<float> cost_tex_d;            // MPPIB_BLOB_COST_TEXTURE: QuadrotorMapCost's map, width * height floats
   mppib_elevation_map_header cost_tex_hdr{};  // use == 0 until a map is set
-  cudaArray_t costmap_array = nullptr;
-  cudaTextureObject_t costmap_tex = 0;
+  ArrayTexture costmap_tex;                   // MPPIB_BLOB_COSTMAP: float4 array + its texture object
 
   // RNG
   curandGenerator_t gen = nullptr;
@@ -161,14 +161,13 @@ struct mppib_engine
   // double-buffered noise: the draw for solve s+1 runs on a side stream while K1/K2 of solve s run (it depends on
   // nothing but the RNG position)
   bool prefetch_enabled = false;
-  float* noise_alloc2 = nullptr;
+  DeviceBuffer<float> noise_alloc2;
   float* eps_buf[2] = { nullptr, nullptr };
   CUtensorMap tmap_buf[2];
   int cur_buf = 0;
-  cudaStream_t side_stream = nullptr;
-  cudaEvent_t ev_k1_done[2] = { nullptr, nullptr };   // K1 that read eps_buf[i] has finished
-  cudaEvent_t ev_gen_done[2] = { nullptr, nullptr };  // the draw into eps_buf[i] has finished
-  cudaEvent_t ev_last_gen = nullptr;                   // last draw on either stream (generator state ordering)
+  Event ev_k1_done[2];   // K1 that read eps_buf[i] has finished
+  Event ev_gen_done[2];  // the draw into eps_buf[i] has finished
+  Event ev_last_gen;     // last draw on either stream (generator state ordering)
   bool k1_recorded[2] = { false, false };
   bool any_gen = false;
   bool prefetch_valid = false;
@@ -186,39 +185,38 @@ struct mppib_engine
   // ColoredNoise sampler (noise_colored.cuh)
   bool colored = false;
   bool nln = false;              // NLN sampler: C log-normal planes + one normal block per draw (nln.cu:114-128)
-  float* nln_d = nullptr;        // [C][N][T]
+  DeviceBuffer<float> nln_d;     // [C][N][T]
   int F = 0;                     // T + 1 frequencies
   float2* spec_d = nullptr;      // [n_local*C][F] complex spectrum == the raw draw
-  float* spec_alloc = nullptr;   // allocation incl. the offset-alignment lead-in
-  float* time_d = nullptr;       // [n_local*C][2T] cuFFT output, kept until the next draw
-  float* coeffs_d = nullptr;     // [C][F]
-  float* sigma_d = nullptr;      // [C]
-  float* decay_pow_d = nullptr;  // [T] powf(offset_decay_rate, t)
+  DeviceBuffer<float> spec_alloc;   // allocation incl. the offset-alignment lead-in
+  DeviceBuffer<float> time_d;       // [n_local*C][2T] cuFFT output, kept until the next draw
+  DeviceBuffer<float> coeffs_d;     // [C][F]
+  DeviceBuffer<float> sigma_d;      // [C]
+  DeviceBuffer<float> decay_pow_d;  // [T] powf(offset_decay_rate, t)
   cufftHandle fft_plan = 0;
   bool have_plan = false;
   int colored_offset_t = 1;      // optimization_stride assumed by draws issued before a solve names its own
   int buf_offset_t[2] = { 1, 1 };  // stride the colored block in eps_buf[i] was rearranged with
-  cudaEvent_t ev_rearr = nullptr;  // last re-rearrange on the main stream (time_d must outlive it)
+  Event ev_rearr;                  // last re-rearrange on the main stream (time_d must outlive it)
   bool rearr_recorded = false;
-  uint32_t* xw_states_d = nullptr;
-  uint32_t* xw_tables_d = nullptr;
+  DeviceBuffer<uint32_t> xw_states_d;
+  DeviceBuffer<uint32_t> xw_tables_d;
 
   // device buffers
-  float* noise_alloc = nullptr;  // allocation incl. lead-in space for offset alignment
-  float* eps_d = nullptr;        // [n_local][T][C]
-  float* costs_d = nullptr;      // [D][n_local]
-  float* partials_d = nullptr;   // [grid][D][pstride]
-  float4* headers_d = nullptr;   // [grid][D] compact (beta, eta, sum w^2)
-  float4* gather_hdr_d = nullptr;  // [world][D]
-  float* controls_d = nullptr;   // optional [D][n_local][T][C]
-  float* rank_rec_d = nullptr;   // [D][pstride] this rank's record (world > 1)
-  float* gather_d = nullptr;     // [world][D][pstride]
-  float* result_d = nullptr;     // [D][pstride] final record (device copy)
-  float* result_h = nullptr;     // mapped pinned host copy K2 writes directly
-  float* result_h_dev = nullptr; // device alias of result_h
-  float* weights_d = nullptr;    // lazily allocated for mppib_get_weights
-  unsigned char* l2_flush_d = nullptr;  // optional: buffer written between K0 and K1 to evict the noise from L2
-  size_t l2_flush_bytes = 0;
+  DeviceBuffer<float> noise_alloc;    // allocation incl. lead-in space for offset alignment
+  float* eps_d = nullptr;             // [n_local][T][C]
+  DeviceBuffer<float> costs_d;        // [D][n_local]
+  DeviceBuffer<float> partials_d;     // [grid][D][pstride]
+  DeviceBuffer<float4> headers_d;     // [grid][D] compact (beta, eta, sum w^2)
+  DeviceBuffer<float4> gather_hdr_d;  // [world][D]
+  DeviceBuffer<float> controls_d;     // optional [D][n_local][T][C]
+  DeviceBuffer<float> rank_rec_d;     // [D][pstride] this rank's record (world > 1)
+  DeviceBuffer<float> gather_d;       // [world][D][pstride]
+  DeviceBuffer<float> result_d;       // [D][pstride] final record (device copy)
+  PinnedBuffer<float> result_h;       // mapped pinned host copy K2 writes directly
+  float* result_h_dev = nullptr;      // device alias of result_h
+  DeviceBuffer<float> weights_d;      // lazily allocated for mppib_get_weights
+  DeviceBuffer<unsigned char> l2_flush_d;  // optional: all of it is written between K0 and K1 to evict the noise from L2
   int pending = 0;               // solves enqueued and not yet waited for
   // accumulated stage timings (timing mode)
   double acc_ms[4] = { 0, 0, 0, 0 };
@@ -231,14 +229,14 @@ struct mppib_engine
   // peer-memory exchange (combine_kernel.cuh: exchange_merge_kernel)
   bool p2p = false;
   bool p2p_opened = false;
-  float* p2p_gather_d = nullptr;   // [2][world][D][pstride] followed by the flag words [2][world]
+  DeviceBuffer<float> p2p_gather_d;  // [2][world][D][pstride] followed by the flag words [2][world]
   PeerTable peers{};
   void* peer_opened[8] = { nullptr };
   unsigned p2p_seq = 0;
 
   // timing
   bool timing = false;
-  cudaEvent_t ev[4] = { nullptr, nullptr, nullptr, nullptr };
+  Event ev[4];
   bool timing_valid = false;
 
   // registry hook
@@ -417,7 +415,7 @@ struct Pair
     a.costs = e.costs_d;
     a.partials = e.partials_d;
     a.headers = e.headers_d;
-    a.controls_out = e.writeback ? e.controls_d : nullptr;
+    a.controls_out = e.writeback ? e.controls_d.get() : nullptr;
     a.n_local = e.n_local;
     a.n_offset = e.n_offset;
     a.T = e.T;
@@ -483,7 +481,7 @@ static int sampled_traj_launch(mppib_engine& e, const float* x0, const float* U_
   Args a;
   fill_pair_args(a, e, 0);
   a.controls = e.controls_d + (size_t)distribution * e.n_local * e.TC;
-  a.opt = have_opt ? e.vis_opt_d : nullptr;
+  a.opt = have_opt ? e.vis_opt_d.get() : nullptr;
   a.sample_idx = e.vis_idx_d;
   a.outputs = e.vis_outputs_d;
   a.costs = e.vis_costs_d;

@@ -1,0 +1,76 @@
+"""Check that an engine gives back every byte of device memory it took, after each buffer that grows or is freed on
+demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
+  - an RMPPI engine (quadrotor + QuadrotorMapCost, D = 2): solve, init-eval twice with more candidates the second time, the
+    cost map replaced by one with four times the cells, the feedback gains set, freed and set again, a solve after each;
+  - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time.
+The free device memory (cudaMemGetInfo) after both are destroyed is compared with the value before they were created. The
+sequence runs twice and the second pass is the one checked: the first also loads the kernels, which stay on the device.
+Every call raises on a status other than MPPIB_OK. Prints one JSON line; exits 1 if the second pass leaves more than
+`--slack-mib` less free memory than it found (another process on a shared card can move the figure as well).
+Usage: python tools/engine_memory_check.py [--slack-mib 2]"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import mppi_generic_b200 as m  # noqa: E402
+from mppi_generic_b200 import workloads as W  # noqa: E402
+
+H = m.host
+
+
+def exercise():
+    w = W.quadrotor_gates(1024, 40)
+    e = H.Engine(w.dyn, w.cost, w.sampler, w.N, w.T, 2, flags=H.FLAG_RMPPI)
+    e.set_solver(w.dt, w.lambda_, w.alpha)
+    e.seed(w.seed, 0)
+    gains = (np.random.RandomState(3).randn(w.T, 13, 4) * 0.05).astype(np.float32)
+    x0 = np.stack([w.x0[0], w.x0[0] + np.array([0.05, 0.1, 0.02] + [0.0] * 10, np.float32)])
+    U = np.tile(w.U0, (2, 1, 1))
+    e.set_rmppi(3000.0, gains)
+    e.solve(x0, U)
+    for K, spc in ((2, 32), (4, 128)):
+        cand = np.linspace(x0[0], x0[1], K).astype(np.float32)
+        e.init_eval(cand, np.arange(K, dtype=np.int32), spc, U[0], 1)
+    w.cost.tex_helper_ = W.quadrotor_track_map(resolution=0.125)[0]
+    e.push_cost()
+    e.solve(x0, U)
+    e.set_rmppi(3000.0, None)
+    e.solve(x0, U)
+    e.set_rmppi(3000.0, gains)
+    e.solve(x0, U)
+    e.close()
+
+    w = W.quadrotor_gates(1024, 40)
+    e = w.make_engine(flags=H.FLAG_WRITEBACK_CONTROLS)
+    U_opt, _ = e.solve(w.x0, w.U0)
+    for n in (8, 256):
+        idx = np.concatenate([[-1], np.arange(n - 1)]).astype(np.int32)
+        e.sample_trajectories(w.x0[0], w.U0[0], idx, U_opt=U_opt[0])
+    e.close()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--slack-mib", type=float, default=2.0)
+    a = ap.parse_args()
+    torch.cuda.init()
+    free = [torch.cuda.mem_get_info()[0]]
+    for _ in range(2):
+        exercise()
+        free.append(torch.cuda.mem_get_info()[0])
+    out = {"gpu": torch.cuda.get_device_name(0), "free_before": free[0], "free_after_first_pass": free[1],
+           "free_after_second_pass": free[2], "second_pass_kept_bytes": free[1] - free[2]}
+    out["ok"] = out["second_pass_kept_bytes"] <= a.slack_mib * 2 ** 20
+    print(json.dumps(out))
+    sys.exit(0 if out["ok"] else 1)
+
+
+if __name__ == "__main__":
+    main()
