@@ -2,10 +2,12 @@
  * device_resources.cuh — owners of the CUDA resources an engine holds (engine_internal.cuh: mppib_engine). Each one releases
  * what it holds in its destructor, so a resource is one member declaration and no failure path can leak it or free it twice.
  * They live in place inside the engine and are neither copied nor moved; each reads as the raw handle it owns (empty: null).
- * They return cudaError_t, so CUDA_TRY(buf.reserve(n, stream)) reads like any other runtime call.
+ * They return their library's status, so CUDA_TRY(buf.reserve(n, stream)) reads like any other runtime call.
  */
 #pragma once
 #include <cuda_runtime.h>
+#include <cufft.h>
+#include <curand.h>
 
 #include <cstddef>
 #include <utility>
@@ -191,4 +193,31 @@ private:
   cudaArray_t array_ = nullptr;
   cudaTextureObject_t tex_ = 0;
 };
+
+// A cuRAND generator or cuFFT plan, made by a call such as cufftPlan1d(&h, ...) and destroyed only if that call
+// succeeded (a cufftHandle has no null value)
+template <class H, class R, R (*Destroy)(H), R kOk>
+class LibraryHandle : NoCopy
+{
+public:
+  ~LibraryHandle()
+  {
+    if (made_)
+      Destroy(h_);
+  }
+  operator H() const { return h_; }
+  template <class... P, class... A>
+  R make(R (*create)(H*, P...), A... a)
+  {
+    const R r = create(&h_, a...);
+    made_ = r == kOk;
+    return r;
+  }
+
+private:
+  H h_{};
+  bool made_ = false;
+};
+using CurandGenerator = LibraryHandle<curandGenerator_t, curandStatus_t, curandDestroyGenerator, CURAND_STATUS_SUCCESS>;
+using CufftPlan = LibraryHandle<cufftHandle, cufftResult, cufftDestroy, CUFFT_SUCCESS>;
 }  // namespace mppib

@@ -2,8 +2,10 @@
 demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
   - an RMPPI engine (quadrotor + QuadrotorMapCost, D = 2): solve, init-eval twice with more candidates the second time, the
     cost map replaced by one with four times the cells, the feedback gains set, freed and set again, a solve after each;
-  - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time.
-The free device memory (cudaMemGetInfo) after both are destroyed is compared with the value before they were created. The
+  - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time;
+  - a ColoredNoise and an NLN engine (the samplers whose spectrum, plan and log-normal planes the noise source owns): solve,
+    new sampler parameters, solve, burn_draws, solve.
+The free device memory (cudaMemGetInfo) after all four are destroyed is compared with the value before they were created. The
 sequence runs twice and the second pass is the one checked: the first also loads the kernels, which stay on the device.
 Every call raises on a status other than MPPIB_OK. Prints one JSON line; exits 1 if the second pass leaves more than
 `--slack-mib` less free memory than it found (another process on a shared card can move the figure as well).
@@ -54,6 +56,21 @@ def exercise():
         idx = np.concatenate([[-1], np.arange(n - 1)]).astype(np.int32)
         e.sample_trajectories(w.x0[0], w.U0[0], idx, U_opt=U_opt[0])
     e.close()
+
+    # N * T a multiple of 8192: an NLN draw re-positions the generator after burn_draws only on such a boundary
+    for sampler in (H.ColoredNoiseDistribution(2, [1.0, 1.0], [1.0, 2.0]), H.NLNDistribution(2, [0.5, 0.5])):
+        w = W.double_integrator_vanilla(1024, 32)
+        w.sampler = sampler
+        e = w.make_engine()
+        e.solve(w.x0, w.U0)
+        sampler.setStdDev([0.8, 0.6])
+        if isinstance(sampler, H.ColoredNoiseDistribution):
+            sampler.setExponents([0.5, 1.5])
+        e.push_params()
+        e.solve(w.x0, w.U0)
+        e.burn_draws(3)
+        e.solve(w.x0, w.U0)
+        e.close()
 
 
 def main():
