@@ -155,7 +155,7 @@ static int make_tensor_map(mppib_engine& e, float* base, CUtensorMap* out)
     return fail(MPPIB_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t gdim[2] = { (cuuint64_t)e.TC, (cuuint64_t)e.n_local };
   cuuint64_t gstride[1] = { (cuuint64_t)e.TC * sizeof(float) };
-  cuuint32_t box[2] = { (cuuint32_t)kChunkFloats, (cuuint32_t)e.bx };
+  cuuint32_t box[2] = { (cuuint32_t)kChunkFloats, (cuuint32_t)e.k1.bx };
   cuuint32_t estride[2] = { 1, 1 };
   CUresult r = ((EncodeFn)fn)(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstride, box, estride,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -562,7 +562,7 @@ static int launch_combine(mppib_engine& e, bool after_k1)
   if (e.tsallis_gamma != 0.0f && e.tsallis_r != 0.0f)
   {
     // K2 for the global baseline (device copy only), then the Tsallis-weighted reduction of the written-back controls
-    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.grid, 1, e.result_d, nullptr, pdl, false);
+    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 1, e.result_d, nullptr, pdl, false);
     if (rc1 != MPPIB_OK)
       return rc1;
     const dim3 grid((e.TC + 31) / 32, e.D, 1);
@@ -576,14 +576,14 @@ static int launch_combine(mppib_engine& e, bool after_k1)
   }
   if (e.desc.world_size == 1 || !e.comm)
   {
-    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.grid, 1, e.result_d, host_copy, pdl, true);
+    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 1, e.result_d, host_copy, pdl, true);
     if (rc1 == MPPIB_OK && !e.mapped_result)
       CUDA_TRY(cudaMemcpyAsync(e.result_h, e.result_d, (size_t)e.D * e.pstride * sizeof(float), cudaMemcpyDeviceToHost,
                                e.stream));
     return rc1;
   }
   // rank record (un-normalised) -> all-gather -> merge of the world_size records (normalised)
-  int rc = launch_combine_one(e, e.partials_d, e.headers_d, e.grid, 0, e.rank_rec_d, nullptr, pdl);
+  int rc = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 0, e.rank_rec_d, nullptr, pdl);
   if (rc != MPPIB_OK)
     return rc;
   if (e.p2p)
@@ -705,7 +705,8 @@ static K1Overrides read_k1_overrides(const mppib_desc& desc)
 
 // The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
 // tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
-static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairEntry** out)
+// *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that has one, even if NN_MMA then keeps the mma.sync entry.
+static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairEntry** out, bool* wgmma_asked)
 {
   const PairEntry* entry = nullptr;
   for (const auto& p : kPairs)
@@ -714,6 +715,7 @@ static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairE
   for (const PairEntry* p : user_pairs())  // out-of-tree pairs (mppib_load_plugin / mppib_register_pair)
     if (p->dyn_id == desc.dynamics_id && p->cost_id == desc.cost_id)
       entry = p;
+  *wgmma_asked = entry && entry->has_wgmma && ov.nn_tensor;
   // Autorally pair: the network runs on register-level mma.sync by default (plugins/nn_mma.cuh). NN_FFMA2 keeps the FFMA2
   // form, NN_TENSOR selects the wgmma kernel (which is built on the FFMA2 entry).
   if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(ov.nn_ffma2 || ov.nn_tensor) || ov.nn_mma))
@@ -743,58 +745,59 @@ static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairE
   return MPPIB_OK;
 }
 
-// K1's form and launch geometry for an engine whose pair, sizes and flags are set: the generic, SPT = 2, RMPPI, warp-
-// specialised or wgmma kernel, resident or streaming, and bx, threads, grid, shared memory. Pair<>::kernel maps the choice
-// to the instantiation.
-static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides& ov)
+// K1's plan for an engine whose sizes, flags and SM count are set, from its pair entry, the overrides and the device's
+// limits: the generic, SPT = 2, RMPPI, warp-specialised or wgmma kernel, resident or streaming, and bx, threads, grid,
+// shared memory. `wgmma_asked`: NN_TENSOR asks for the wgmma kernel of a pair that has one (pick_entry).
+static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Overrides& ov, bool wgmma_asked, K1Plan* out)
 {
   // One thread per sample; bx samples per CTA, whole-horizon noise tile resident in shared memory. The rollout is bound by
   // the T-step dependency chain, so a CTA takes the same time whatever its width: the block width is chosen to put every CTA
   // in ONE wave (no tail wave running at a fraction of the chip), preferring the narrowest such width (more SMs busy, fewer
   // warps contending per scheduler); 64 if several waves are unavoidable.
-  const mppib_desc& desc = e->desc;
-  int max_smem = 0, num_sms = 0, smem_per_sm = 0;
+  const mppib_desc& desc = e.desc;
+  const int num_sms = e.num_sms;
+  int max_smem = 0, smem_per_sm = 0;
   CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, desc.device));
-  CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, desc.device));
   CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, desc.device));
-  e->num_sms = num_sms;
-  const bool tma_ok = !ov.no_tma && e->TC % 4 == 0;
+  K1Plan p;
+  p.D = e.D;
+  const bool tma_ok = !ov.no_tma && e.TC % 4 == 0;
   // samples per thread (rollout_kernel.cuh): 1. SPT = 2 halves the shared-memory wavefronts per sample of the NN model
   // but a lone warp per scheduler cannot overlap its own FFMA2 / MUFU / latency phases the
   // way two warps do, and it measured slower. Kept selectable for experiments through MPPIB_SPT.
-  e->spt = (ov.spt >= 1 && ov.spt <= entry->max_spt && (ov.spt == 1 || e->D == 1)) ? ov.spt : 1;
-  e->lps = 32 / entry->spw;
-  const int spt = e->spt, lps = e->lps;
+  p.spt = (ov.spt >= 1 && ov.spt <= entry->max_spt && (ov.spt == 1 || e.D == 1)) ? ov.spt : 1;
+  p.lps = 32 / entry->spw;
+  const int spt = p.spt, lps = p.lps;
   // Autorally pair, one system: the warp-specialised K1 (rollout_kernel_ar_ws.cuh) — a producer and a consumer warp per 32
   // samples. MPPIB_NO_WS / MPPIB_SPW / MPPIB_SPT keep the generic kernel (A/B runs, tests of the generic form).
-  const bool is_mma = entry >= kPairsMma && entry < kPairsMma + sizeof(kPairsMma) / sizeof(kPairsMma[0]);
-  e->ar_ws = is_mma && entry->spw == 32 && e->D == 1 && !e->rmppi && spt == 1 && !ov.no_ws && !ov.spw_set;
-  const bool ws = e->ar_ws;
+  const bool ws = entry->has_warp_spec && e.D == 1 && !e.rmppi && spt == 1 && !ov.no_ws && !ov.spw_set;
+  p.form = ws ? K1Form::WarpSpec
+              : (e.rmppi ? K1Form::Rmppi : (e.D == 1 && spt == 2 ? K1Form::GenericSpt2 : K1Form::Generic));
   // samples per producer warp: 16 while the GPU is throughput-bound; 8 (four producers per 32 samples, one per scheduler)
   // once it holds so few rollouts that a group's step time sets K1 (kWsPspw8MaxRollouts)
-  e->ws_pspw = (ov.ws_pspw == 32 || ov.ws_pspw == 16 || ov.ws_pspw == 8) ? ov.ws_pspw
-                                                                        : (e->n_local <= kWsPspw8MaxRollouts ? 8 : 16);
-  const int ws_wpg = ar_ws::warpsPerGroup(e->ws_pspw);
+  p.ws_pspw = (ov.ws_pspw == 32 || ov.ws_pspw == 16 || ov.ws_pspw == 8) ? ov.ws_pspw
+                                                                       : (e.n_local <= kWsPspw8MaxRollouts ? 8 : 16);
+  const int ws_wpg = ar_ws::warpsPerGroup(p.ws_pspw);
   // shared memory of a CTA of b samples whose noise tile holds `chunks` 32-column slabs (all: resident; a ring: streaming)
   auto layout = [&](int b, int chunks) {
-    const int dyn_floats = ws ? ar_ws::sharedFloats(b) : e->dyn_shared_floats_fn(desc.model_dims, b);
-    return (int)rollout_smem_layout(b, chunks, e->D, e->TC, dyn_floats, e->cost_shared_floats(e->T)).total;
+    const int dyn_floats = ws ? ar_ws::sharedFloats(b) : entry->dyn_shared_floats(desc.model_dims, b);
+    return (int)rollout_smem_layout(b, chunks, e.D, e.TC, dyn_floats, entry->cost_shared_floats(e.T)).total;
   };
-  auto smem_for = [&](int b) { return layout(b, e->nchunks); };
+  auto smem_for = [&](int b) { return layout(b, e.nchunks); };
   const int unit = ws ? 32 : entry->spw * spt;  // samples per warp of threads
-  const int max_bx = ws ? 32 * ar_ws::maxGroups(e->ws_pspw) : entry->max_block_threads / 32 * unit;  // samples per CTA (__launch_bounds__)
+  const int max_bx = ws ? 32 * ar_ws::maxGroups(p.ws_pspw) : entry->max_block_threads / 32 * unit;  // samples per CTA (__launch_bounds__)
   auto threads_for = [&](int b) { return ws ? ws_wpg * b : b / spt * lps; };
   // resident CTAs per SM: shared memory (+1 KB the hardware reserves per CTA), threads, and for the warp-specialised kernel
   // its 128-register budget
   auto ctas_per_sm = [&](int b, int sm) {
     int n = std::min(std::min(smem_per_sm / (sm + 1024), 2048 / threads_for(b)), 32);
     if (ws)  // registers: __launch_bounds__(maxThreads, 1) lets ptxas use 65536 / maxThreads per thread
-      n = std::min(n, ar_ws::maxThreads(e->ws_pspw) / threads_for(b));
+      n = std::min(n, ar_ws::maxThreads(p.ws_pspw) / threads_for(b));
     return n;
   };
   auto waves = [&](int b, int per_sm) {  // waves of CTAs of b samples at per_sm CTAs per SM
     const long per_wave = (long)per_sm * num_sms;
-    return ((e->n_local + b - 1) / b + per_wave - 1) / per_wave;
+    return ((e.n_local + b - 1) / b + per_wave - 1) / per_wave;
   };
   int bx = ov.bx;  // MPPIB_BX, up to 512 here and clamped to max_bx below
   if (bx < unit || bx > 512 || (bx % unit) != 0)
@@ -806,12 +809,12 @@ static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides&
     // beyond that ONE CTA per SM, as narrow as covers n_local, so that every SM is busy and the kernel's alternating role
     // table (P C C P C P P C) balances producers over the four schedulers. Wider than the resident tile fits: the wave rule
     // below, and then the streaming form at this width.
-    const long pairs_total = (e->n_local + 31) / 32;
+    const long pairs_total = (e.n_local + 31) / 32;
     if (ws_wpg * pairs_total <= 4L * num_sms)
       bx = 32;
     else
     {
-      const int need = (int)(((e->n_local + num_sms - 1) / num_sms + 31) / 32) * 32;
+      const int need = (int)(((e.n_local + num_sms - 1) / num_sms + 31) / 32) * 32;
       if (need <= max_bx)
         ws_one_wave = need;
       if (need <= max_bx && smem_for(need) <= max_smem)
@@ -846,19 +849,23 @@ static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides&
     bx = unit;
   while (smem_for(bx) > max_smem && bx > unit)
     bx -= unit;
-  e->smem_bytes = (uint32_t)smem_for(bx);
-  if ((int)e->smem_bytes > max_smem)
-    return fail(MPPIB_ERR_SMEM, "noise tile needs %u B of shared memory, device allows %d", e->smem_bytes, max_smem);
+  p.smem_bytes = (uint32_t)smem_for(bx);
+  if ((int)p.smem_bytes > max_smem)
+    return fail(MPPIB_ERR_SMEM, "noise tile needs %u B of shared memory, device allows %d", p.smem_bytes, max_smem);
   // tensor-core variant of the Autorally pair: fixed 128-sample CTAs (one warpgroup, two m64 wgmma tiles), streaming
-  // noise ring. Opt-in: three exposed MMA round trips per step with few warps per SM to cover them
-  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc.cost_id == MPPIB_COST_AR_STANDARD && e->D == 1 && tma_ok &&
-      ov.nn_tensor)
+  // noise ring. Opt-in: three exposed MMA round trips per step with few warps per SM to cover them.
+  // MPPIB_FLAG_NN_MMA with NN_TENSOR keeps the mma.sync entry (pick_entry), which has no wgmma kernel: the form chosen
+  // above launches, at the wgmma kernel's width and shared memory (streaming only in the warp-specialised form). This is
+  // deliberate: the flag combination keeps the launch it has always had.
+  const bool wgmma_width = wgmma_asked && e.D == 1 && tma_ok;
+  if (wgmma_width)
   {
-    e->nn_tc = true;
+    if (entry->has_wgmma)
+      p.form = K1Form::Wgmma;
     bx = nn_tc::kRows;
-    e->smem_bytes = nn_tc::layout(e->TC, e->T).total;
-    if ((int)e->smem_bytes > max_smem)
-      return fail(MPPIB_ERR_SMEM, "tensor-core rollout needs %u B of shared memory, device allows %d", e->smem_bytes,
+    p.smem_bytes = nn_tc::layout(e.TC, e.T).total;
+    if ((int)p.smem_bytes > max_smem)
+      return fail(MPPIB_ERR_SMEM, "tensor-core rollout needs %u B of shared memory, device allows %d", p.smem_bytes,
                   max_smem);
   }
   // Streaming form (STREAM in rollout_kernel.cuh and rollout_kernel_ar_ws.cuh): the noise slabs cycle through a ring, so
@@ -869,16 +876,16 @@ static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides&
   // fit, and the 96-thread CTAs the wave rule falls back to run in two waves); forced, it also runs without TMA (the issuing
   // warp fills the ring with plain loads).
   {
-    const int ring = ws ? ar_ws::kNoiseRing : e->ring;
+    const int ring = ws ? ar_ws::kNoiseRing : p.ring;
     const bool env_bx_ok = ov.bx >= unit && ov.bx <= max_bx && (ov.bx % unit) == 0;
     const int sbx = ws ? ((ws_one_wave && !ov.bx_set) ? ws_one_wave : bx) : (env_bx_ok ? ov.bx : 64);
     const int sm_str = layout(sbx, ring);
-    const bool auto_ok = tma_ok && e->nchunks > ring;
-    if ((ws || (auto_ok && !e->rmppi && !e->nn_tc && spt == 1)) && sm_str <= max_smem)
+    const bool auto_ok = tma_ok && e.nchunks > ring;
+    if ((ws || (auto_ok && !e.rmppi && !wgmma_width && spt == 1)) && sm_str <= max_smem)
     {
       // the generic kernel asks the occupancy API (registers count too); the warp-specialised one's budget is fixed
       const int per_sm_str = ws ? std::max(1, ctas_per_sm(sbx, sm_str))
-                                : entry->stream_blocks_per_sm(*e, threads_for(sbx), (size_t)sm_str);
+                                : entry->stream_blocks_per_sm(p, threads_for(sbx), (size_t)sm_str);
       if (per_sm_str > 0)
       {
         const long waves_res = waves(bx, std::max(1, ctas_per_sm(bx, smem_for(bx))));
@@ -887,25 +894,24 @@ static int choose_k1(mppib_engine* e, const PairEntry* entry, const K1Overrides&
           want = ov.stream;
         if (want)
         {
-          e->stream_k1 = true;
-          if (!ws && ov.stream_readback)  // A/B: the round-1 form (controls written back and re-read by the epilogue)
-            e->writeback = true;
+          p.stream = true;
+          // A/B: the round-1 form, controls written back and re-read by the epilogue (mppib_create turns write-back on)
+          p.stream_readback = !ws && ov.stream_readback;
           bx = sbx;
-          e->smem_bytes = (uint32_t)sm_str;
+          p.smem_bytes = (uint32_t)sm_str;
         }
       }
     }
   }
-  e->bx = bx;
-  // MPPIB_FLAG_NN_MMA with NN_TENSOR keeps the mma.sync entry, which has no wgmma kernel: Pair<>::kernel runs another form
-  e->threads = (e->nn_tc && !is_mma) ? nn_tc::kRows : threads_for(bx);
-  e->dyn_shared_floats = ws ? ar_ws::sharedFloats(bx) : e->dyn_shared_floats_fn(desc.model_dims, bx);
-  e->grid = (e->n_local + bx - 1) / bx;
-  if (e->grid > kCombineMaxRecords)
-    return fail(MPPIB_ERR_UNSUPPORTED, "%d rollout blocks exceed the combine kernel's %d records; raise MPPIB_BX", e->grid,
+  p.bx = bx;
+  p.threads = p.form == K1Form::Wgmma ? nn_tc::kRows : threads_for(bx);
+  p.dyn_shared_floats = ws ? ar_ws::sharedFloats(bx) : entry->dyn_shared_floats(desc.model_dims, bx);
+  p.grid = (e.n_local + bx - 1) / bx;
+  if (p.grid > kCombineMaxRecords)
+    return fail(MPPIB_ERR_UNSUPPORTED, "%d rollout blocks exceed the combine kernel's %d records; raise MPPIB_BX", p.grid,
                 kCombineMaxRecords);
-  e->use_tma = tma_ok;
-  e->stream_readback = e->stream_k1 && e->writeback && ov.stream_readback;
+  p.use_tma = tma_ok;
+  *out = p;
   return MPPIB_OK;
 }
 
@@ -933,10 +939,10 @@ int mppib_register_pair(const void* pair_entry, size_t entry_bytes, unsigned abi
                 in->cost_id);
   if (in->C != 1 && in->C != 2 && in->C != 4)
     return fail(MPPIB_ERR_UNSUPPORTED, "CONTROL_DIM %d: must divide a 16-byte noise group (1, 2 or 4)", in->C);
-  for (PairEntry* p : user_pairs())
+  for (PairEntry*& p : user_pairs())
     if (p->dyn_id == in->dyn_id && p->cost_id == in->cost_id)
     {
-      *p = *in;  // re-registration (plugin reloaded)
+      p = new PairEntry(*in);  // re-registration (plugin reloaded): engines made from the old entry keep it
       return MPPIB_OK;
     }
   user_pairs().push_back(new PairEntry(*in));
@@ -1043,7 +1049,8 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
       return fail(MPPIB_ERR_UNSUPPORTED, "RacerDubinsElevationLSTMSteering is built for num_distributions == 1 only");
   }
   const PairEntry* entry = nullptr;
-  if (int rc = pick_entry(*desc, ov, &entry))
+  bool wgmma_asked = false;
+  if (int rc = pick_entry(*desc, ov, &entry, &wgmma_asked))
     return rc;
 
   int ndev = 0;
@@ -1067,16 +1074,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   e->N = desc->num_rollouts;
   e->T = desc->num_timesteps;
   e->TC = e->T * e->C;
-  e->launch_rollout = entry->launch;
-  e->prepare = entry->prepare;
-  e->init_eval = entry->init_eval;
-  e->sampled_traj = entry->sampled_traj;
-  e->nominal_traj = entry->nominal_traj;
-  e->ddp = entry->ddp;
-  e->dyn_param_bytes = entry->dyn_bytes;
-  e->cost_param_bytes = entry->cost_bytes;
-  e->dyn_shared_floats_fn = entry->dyn_shared_floats;
-  e->cost_shared_floats = entry->cost_shared_floats;
+  e->pair = entry;
   e->rmppi = (desc->flags & MPPIB_FLAG_RMPPI) != 0;
   if (e->rmppi && desc->num_distributions != 2)
     return fail(MPPIB_ERR_INVALID_ARG, "MPPIB_FLAG_RMPPI needs num_distributions == 2 (nominal, real)");
@@ -1100,8 +1098,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (e->n_local <= 0)
     return fail(MPPIB_ERR_INVALID_ARG, "rank %d of %d has no rollouts (N=%d)", desc->rank, world, e->N);
 
-  if (int rc = choose_k1(e, entry, ov))
+  CUDA_TRY(cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, desc->device));
+  if (int rc = choose_k1(*e, entry, ov, wgmma_asked, &e->k1))
     return rc;
+  if (e->k1.stream_readback)
+    e->writeback = true;
   e->pstride = ((kPartialHeader + e->TC + 3) / 4) * 4;
 
   int prio_lo = 0, prio_hi = 0;
@@ -1114,8 +1115,8 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (int rc = e->noise.create(e->desc, e->N, e->n_offset, e->n_local, e->T, e->C, e->num_sms, e->stream, prio_lo))
     return rc;
   CUDA_TRY(e->costs_d.alloc((size_t)e->D * e->n_local));
-  CUDA_TRY(e->partials_d.alloc((size_t)e->grid * e->D * e->pstride));
-  CUDA_TRY(e->headers_d.alloc((size_t)e->grid * e->D));
+  CUDA_TRY(e->partials_d.alloc((size_t)e->k1.grid * e->D * e->pstride));
+  CUDA_TRY(e->headers_d.alloc((size_t)e->k1.grid * e->D));
   CUDA_TRY(e->result_d.alloc((size_t)e->D * e->pstride));
   CUDA_TRY(e->result_h.alloc((size_t)e->D * e->pstride, cudaHostAllocMapped, &e->result_h_dev));
   memset(e->result_h, 0, (size_t)e->D * e->pstride * sizeof(float));
@@ -1134,11 +1135,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   for (int i = 0; i < 4; i++)
     CUDA_TRY(e->ev[i].create());
 
-  if (e->use_tma)
+  if (e->k1.use_tma)
     for (int i = 0; i < 2; i++)
       if (int rc = make_tensor_map(*e, e->noise.buffer(i), &e->tmap[i]))
         return rc;
-  if (int rc = e->prepare(*e))
+  if (int rc = entry->prepare(*e))
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
   *out = owner.release();
@@ -1212,15 +1213,15 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
   switch (which)
   {
     case MPPIB_BLOB_DYN_PARAMS:
-      if (nbytes != e->dyn_param_bytes)
+      if (nbytes != e->pair->dyn_bytes)
         return fail(MPPIB_ERR_INVALID_ARG, "dynamics params: got %zu bytes, expected %zu", nbytes,
-                    e->dyn_param_bytes);
+                    e->pair->dyn_bytes);
       e->dyn_blob.assign((const unsigned char*)host, (const unsigned char*)host + nbytes);
       e->have_dyn = true;
       return MPPIB_OK;
     case MPPIB_BLOB_COST_PARAMS:
-      if (nbytes != e->cost_param_bytes)
-        return fail(MPPIB_ERR_INVALID_ARG, "cost params: got %zu bytes, expected %zu", nbytes, e->cost_param_bytes);
+      if (nbytes != e->pair->cost_bytes)
+        return fail(MPPIB_ERR_INVALID_ARG, "cost params: got %zu bytes, expected %zu", nbytes, e->pair->cost_bytes);
       e->cost_blob.assign((const unsigned char*)host, (const unsigned char*)host + nbytes);
       e->have_cost = true;
       return MPPIB_OK;
@@ -1483,7 +1484,7 @@ int mppib_rollout_only(mppib_engine* e, const float* x0, const float* U_in, int 
   if (!x0 || !U_in)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = e->launch_rollout(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = e->pair->launch(*e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -1519,7 +1520,7 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
     CUDA_TRY(cudaMemsetAsync(e->l2_flush_d, 0, e->l2_flush_d.capacity(), e->stream));
   if (e->timing)
     CUDA_TRY(cudaEventRecord(e->ev[1], e->stream));
-  rc = e->launch_rollout(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = e->pair->launch(*e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   rc = e->noise.prefetch();
@@ -1746,7 +1747,7 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
 {
   if (!e || !x0 || !x_target || !u_target)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (!e->ddp)
+  if (!e->pair->ddp)
     return fail(MPPIB_ERR_UNSUPPORTED, "dynamics %d has no analytic Jacobian (computeGrad): no DDP kernel is built for it",
                 e->desc.dynamics_id);
   if (T < 2)
@@ -1786,7 +1787,7 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
   CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
   // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
   CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  int rc = e->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d.get() : nullptr);
+  int rc = e->pair->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d.get() : nullptr);
   if (rc != MPPIB_OK)
     return rc;
   int status = 0;
@@ -1833,8 +1834,8 @@ int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides
   rc = e->noise.draw(optimization_stride);  // sampler_->generateSamples(stride, 0, gen_) (:595)
   if (rc != MPPIB_OK)
     return rc;
-  rc = e->init_eval(*e, e->eval_states_d, e->eval_strides_d, num_candidates, samples_per_candidate, U_nominal,
-                    optimization_stride);
+  rc = e->pair->init_eval(*e, e->eval_states_d, e->eval_strides_d, num_candidates, samples_per_candidate, U_nominal,
+                          optimization_stride);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(e->noise.read_by_kernel());  // the kernel above read the noise: later draws into its buffer wait for it
@@ -1884,7 +1885,7 @@ int mppib_sample_trajectories(mppib_engine* e, const float* x0, const float* U_n
   CUDA_TRY(cudaMemcpyAsync(e->vis_idx_d, sample_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, e->stream));
   if (have_opt)
     CUDA_TRY(cudaMemcpyAsync(e->vis_opt_d, U_opt, (size_t)e->TC * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  rc = e->sampled_traj(*e, x0, U_nominal, distribution, n, have_opt);
+  rc = e->pair->sampled_traj(*e, x0, U_nominal, distribution, n, have_opt);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaMemcpyAsync(outputs, e->vis_outputs_d, (size_t)n * e->T * e->O * sizeof(float), cudaMemcpyDeviceToHost,
@@ -1928,7 +1929,7 @@ int mppib_nominal_trajectory(mppib_engine* e, const float* x0, const float* U, c
     u_src = e->nom_u_d;
     u_stride = e->TC;
   }
-  rc = e->nominal_traj(*e, x0, u_src, u_stride, control_history);
+  rc = e->pair->nominal_traj(*e, x0, u_src, u_stride, control_history);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaMemcpyAsync(e->nom_h, e->nom_d, (n_u + n_s + n_o) * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
@@ -2055,13 +2056,13 @@ int mppib_get_launch_info(mppib_engine* e, int* grid, int* block, int* smem_byte
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
   if (grid)
-    *grid = e->grid;
+    *grid = e->k1.grid;
   if (block)
-    *block = e->threads;
+    *block = e->k1.threads;
   if (smem_bytes)
-    *smem_bytes = (int)e->smem_bytes;
+    *smem_bytes = (int)e->k1.smem_bytes;
   if (uses_tma)
-    *uses_tma = e->use_tma ? 1 : 0;
+    *uses_tma = e->k1.use_tma ? 1 : 0;
   if (kernels_per_solve)  // [K0] + K1 + K2 (+ K2'); cuRAND's own launches are not counted
     *kernels_per_solve = ((e->desc.world_size > 1) ? 3 : 2) + (e->noise.own_kernel() ? 1 : 0);
   return MPPIB_OK;
