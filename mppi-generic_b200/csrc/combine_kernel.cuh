@@ -30,10 +30,7 @@ __global__ void __launch_bounds__(kCombineCols* kCombineGroups)
                    const float4* __restrict__ headers,  // [nrec][D] (beta_b, eta_b, sum w^2_b, -)
                    int nrec, int D, int TC, int pstride, float lambda_inv, int normalize,
                    float* __restrict__ out,    // [D][pstride] (device)
-                   float* __restrict__ out2,   // optional second copy (mapped host result), may be nullptr
-                   unsigned* __restrict__ block_counter,       // device, zero between launches
-                   volatile unsigned* __restrict__ done_flag,  // mapped host word, receives `seq` when out2 is complete
-                   unsigned seq)
+                   float* __restrict__ out2)   // optional second copy (mapped host result), may be nullptr
 {
   __shared__ float scale_sh[kCombineMaxRecords];  // s_b = expf(-(beta_b - beta)/lambda)
   __shared__ float red_f[kCombineGroups];
@@ -160,24 +157,6 @@ __global__ void __launch_bounds__(kCombineCols* kCombineGroups)
         o2[1] = eta_f;
         o2[2] = (float)w2_sh;
         o2[3] = 0.0f;
-      }
-    }
-    // completion flag for the host's spin-wait. Only this warp wrote output; its lane 0 publishes after a system fence
-    // (cumulative over the warp's writes through __syncwarp), and the last block to arrive sets the host word.
-    if (done_flag != nullptr)
-    {
-      __syncwarp();
-      if (lane == 0)
-      {
-        __threadfence_system();
-        const unsigned total = gridDim.x * gridDim.y;
-        const unsigned prev = atomicAdd(block_counter, 1u);
-        if (prev == total - 1)
-        {
-          *block_counter = 0u;
-          __threadfence_system();
-          *done_flag = seq;
-        }
       }
     }
   }

@@ -41,7 +41,6 @@
 namespace
 {
 // ---- minimal NCCL binding, resolved lazily with dlopen so single-GPU users need no NCCL at all --------------------
-typedef struct ncclComm* ncclComm_t;
 struct NcclUniqueId
 {
   char internal[128];
@@ -521,105 +520,206 @@ int NoiseSource::prefetch()
   return MPPIB_OK;
 }
 
-// K2 launch. `pdl` = programmatic dependent launch: the grid may start while the preceding kernel on the stream (K1) is
-// still running and blocks at griddepcontrol.wait until that kernel has completed — hides K2's launch latency.
-static int launch_combine_one(mppib_engine& e, const float* records, const float4* headers, int nrec, int normalize,
-                              float* out, float* out2, bool pdl, bool final_stage = false)
+// ---- the merge (reduction.cuh) ------------------------------------------------------------------------------------
+// A kernel launch on `s`. `pdl` = programmatic dependent launch: the grid may start while the preceding kernel on the
+// stream is still running and blocks at griddepcontrol.wait until that kernel has completed, which hides its launch latency.
+template <class... P, class... A>
+static cudaError_t launch_on(cudaStream_t s, bool pdl, void (*kernel)(P...), dim3 grid, dim3 block, A... args)
 {
-  unsigned* counter = e.k2_counter_d;
-  volatile unsigned* flag = nullptr;
-  unsigned seq = 0;
-  if (final_stage && e.spin_wait && out2 != nullptr)
-  {
-    flag = e.done_flag_dev;
-    seq = ++e.solve_seq;
-    e.flag_armed = true;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((e.TC + kCombineCols - 1) / kCombineCols, e.D, 1);
-  cfg.blockDim = dim3(kCombineCols * kCombineGroups, 1, 1);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = e.stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.stream = s;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  const float lambda_inv = (float)(1.0 / e.lambda);
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, combine_kernel, records, headers, nrec, e.D, e.TC, e.pstride, lambda_inv, normalize,
-                              out, out2, counter, flag, seq));
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
+int Reduction::create(int D, int TC, int grid, int world, int rank, cudaStream_t stream)
+{
+  D_ = D;
+  TC_ = TC;
+  grid_ = grid;
+  world_ = world;
+  rank_ = rank;
+  stream_ = stream;
+  pstride_ = ((kPartialHeader + TC + 3) / 4) * 4;
+  const size_t rec = (size_t)D * pstride_;
+  CUDA_TRY(partials_.alloc((size_t)grid * rec));
+  CUDA_TRY(headers_.alloc((size_t)grid * D));
+  CUDA_TRY(result_.alloc(rec));
+  CUDA_TRY(result_h_.alloc(rec, cudaHostAllocMapped, &result_h_dev_));
+  memset(result_h_, 0, rec * sizeof(float));
+  if (world > 1)
+  {
+    CUDA_TRY(rank_rec_.alloc(rec));
+    CUDA_TRY(gather_.alloc((size_t)world * rec));
+    CUDA_TRY(gather_hdr_.alloc((size_t)world * D));
+  }
   return MPPIB_OK;
 }
 
-static int launch_combine(mppib_engine& e, bool after_k1)
+// What runs after the engine has drained the stream; the buffers follow.
+Reduction::~Reduction()
 {
-  // only a final-stage K2 publishes the completion flag; the Tsallis reduction and the peer-memory exchange kernel end the
-  // solve without it, and wait_for_stream then falls back to cudaStreamSynchronize instead of trusting a stale flag
-  e.flag_armed = false;
-  const bool pdl = after_k1 && e.use_pdl;
-  float* host_copy = e.mapped_result ? e.result_h_dev : nullptr;
-  if (e.tsallis_gamma != 0.0f && e.tsallis_r != 0.0f)
+  if (comm_ && g_nccl.CommDestroy)
+    g_nccl.CommDestroy(comm_);
+  for (void* p : peer_opened_)
+    if (p)
+      cudaIpcCloseMemHandle(p);
+}
+
+int Reduction::enqueue(bool after_k1, const float* costs, const float* controls, int n_local, float lambda)
+{
+  const float lambda_inv = (float)(1.0 / lambda);
+  // K2 over nrec records: out (device) and, when given, out2 (the mapped host copy)
+  auto k2 = [&](const float* records, const float4* headers, int nrec, int normalize, float* out, float* out2, bool pdl) {
+    return launch_on(stream_, pdl, combine_kernel, dim3((TC_ + kCombineCols - 1) / kCombineCols, D_),
+                     dim3(kCombineCols * kCombineGroups), records, headers, nrec, D_, TC_, pstride_, lambda_inv, normalize,
+                     out, out2);
+  };
+  if (tsallis_gamma_ != 0.0f && tsallis_r_ != 0.0f)
   {
     // K2 for the global baseline (device copy only), then the Tsallis-weighted reduction of the written-back controls
-    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 1, e.result_d, nullptr, pdl, false);
-    if (rc1 != MPPIB_OK)
-      return rc1;
-    const dim3 grid((e.TC + 31) / 32, e.D, 1);
-    tsallis_reduce_kernel<<<grid, 512, 0, e.stream>>>(e.costs_d, e.controls_d, e.n_local, e.D, e.TC, e.pstride,
-                                                      e.tsallis_gamma, e.tsallis_r, e.result_d, host_copy);
+    CUDA_TRY(k2(partials_, headers_, grid_, 1, result_, nullptr, after_k1));
+    tsallis_reduce_kernel<<<dim3((TC_ + 31) / 32, D_), 512, 0, stream_>>>(costs, controls, n_local, D_, TC_, pstride_,
+                                                                          tsallis_gamma_, tsallis_r_, result_,
+                                                                          result_h_dev_);
     CUDA_TRY(cudaGetLastError());
-    if (!e.mapped_result)
-      CUDA_TRY(cudaMemcpyAsync(e.result_h, e.result_d, (size_t)e.D * e.pstride * sizeof(float), cudaMemcpyDeviceToHost,
-                               e.stream));
     return MPPIB_OK;
   }
-  if (e.desc.world_size == 1 || !e.comm)
+  if (world_ == 1)
   {
-    int rc1 = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 1, e.result_d, host_copy, pdl, true);
-    if (rc1 == MPPIB_OK && !e.mapped_result)
-      CUDA_TRY(cudaMemcpyAsync(e.result_h, e.result_d, (size_t)e.D * e.pstride * sizeof(float), cudaMemcpyDeviceToHost,
-                               e.stream));
-    return rc1;
-  }
-  // rank record (un-normalised) -> all-gather -> merge of the world_size records (normalised)
-  int rc = launch_combine_one(e, e.partials_d, e.headers_d, e.k1.grid, 0, e.rank_rec_d, nullptr, pdl);
-  if (rc != MPPIB_OK)
-    return rc;
-  if (e.p2p)
-  {  // KX: push to peers over NVLink, wait for theirs, merge — one launch
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(1, 1, 1);
-    cfg.blockDim = dim3(512, 1, 1);
-    cfg.stream = e.stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = e.use_pdl ? 1 : 0;
-    const unsigned seq = ++e.p2p_seq;
-    const float lambda_inv = (float)(1.0 / e.lambda);
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, exchange_merge_kernel, (const float*)e.rank_rec_d, e.peers, e.desc.world_size,
-                                e.desc.rank, e.D, e.TC, e.pstride, lambda_inv, seq, e.result_d, host_copy));
-    if (!e.mapped_result)
-      CUDA_TRY(cudaMemcpyAsync(e.result_h, e.result_d, (size_t)e.D * e.pstride * sizeof(float), cudaMemcpyDeviceToHost,
-                               e.stream));
+    CUDA_TRY(k2(partials_, headers_, grid_, 1, result_, result_h_dev_, after_k1));
     return MPPIB_OK;
   }
-  const size_t rec_floats = (size_t)e.D * e.pstride;
-  rc = g_nccl.AllGather(e.rank_rec_d, e.gather_d, rec_floats, kNcclFloat, e.comm, e.stream);
+  // rank record (un-normalised) -> exchange -> merge of the world_ records (normalised)
+  CUDA_TRY(k2(partials_, headers_, grid_, 0, rank_rec_, nullptr, after_k1));
+  if (p2p_)
+  {  // KX: push to peers over NVLink, wait for theirs, merge — one launch
+    CUDA_TRY(launch_on(stream_, true, exchange_merge_kernel, dim3(1), dim3(512), (const float*)rank_rec_, peers_, world_,
+                       rank_, D_, TC_, pstride_, lambda_inv, ++p2p_seq_, (float*)result_, result_h_dev_));
+    return MPPIB_OK;
+  }
+  const int rc = g_nccl.AllGather(rank_rec_, gather_, (size_t)D_ * pstride_, kNcclFloat, comm_, stream_);
   if (rc != 0)
     return fail(MPPIB_ERR_NCCL, "ncclAllGather failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?");
-  const int nh = e.desc.world_size * e.D;
-  record_headers_kernel<<<(nh + 63) / 64, 64, 0, e.stream>>>(e.gather_d, e.desc.world_size, e.D, e.pstride,
-                                                            e.gather_hdr_d);
+  const int nh = world_ * D_;
+  record_headers_kernel<<<(nh + 63) / 64, 64, 0, stream_>>>(gather_, world_, D_, pstride_, gather_hdr_);
   CUDA_TRY(cudaGetLastError());
-  rc = launch_combine_one(e, e.gather_d, e.gather_hdr_d, e.desc.world_size, 1, e.result_d, host_copy, false, true);
-  if (rc == MPPIB_OK && !e.mapped_result)
-    CUDA_TRY(cudaMemcpyAsync(e.result_h, e.result_d, (size_t)e.D * e.pstride * sizeof(float), cudaMemcpyDeviceToHost,
-                             e.stream));
-  return rc;
+  CUDA_TRY(k2(gather_, gather_hdr_, world_, 1, result_, result_h_dev_, false));
+  return MPPIB_OK;
+}
+
+void Reduction::read(float* U_out, mppib_solve_stats* stats) const
+{
+  for (int d = 0; d < D_; d++)
+  {
+    const float* r = result_h_ + (size_t)d * pstride_;
+    if (stats)
+    {
+      stats[d].baseline = r[0];
+      stats[d].normalizer = r[1];
+      stats[d].sum_w2 = r[2];
+      stats[d].pad = 0.0f;
+    }
+    if (U_out)
+      memcpy(U_out + (size_t)d * TC_, r + kPartialHeader, sizeof(float) * TC_);
+  }
+}
+
+int Reduction::set_tsallis(float gamma, float r, bool have_controls)
+{
+  if (gamma != 0.0f && r != 0.0f)
+  {
+    if (!have_controls)
+      return fail(MPPIB_ERR_STATE, "Tsallis weights reduce the written-back controls: create the engine with "
+                                   "MPPIB_FLAG_WRITEBACK_CONTROLS");
+    if (world_ != 1)
+      return fail(MPPIB_ERR_UNSUPPORTED, "Tsallis weights are built for one rank");
+    if (r == 1.0f || !(gamma > 0.0f))
+      return fail(MPPIB_ERR_INVALID_ARG, "Tsallis weights need gamma > 0 and r != 1");
+  }
+  tsallis_gamma_ = gamma;
+  tsallis_r_ = r;
+  return MPPIB_OK;
+}
+
+int Reduction::comm_init(const void* unique_id_128)
+{
+  if (world_ <= 1)
+    return MPPIB_OK;
+  if (!g_nccl.load())
+    return fail(MPPIB_ERR_NCCL, "libnccl.so.2 could not be loaded: %s", dlerror());
+  NcclUniqueId id;
+  memcpy(&id, unique_id_128, sizeof(id));
+  int rc = g_nccl.CommInitRank(&comm_, world_, id, rank_);
+  if (rc != 0)
+    return fail(MPPIB_ERR_NCCL, "ncclCommInitRank failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?");
+  return MPPIB_OK;
+}
+
+int Reduction::p2p_handle(void* handle_64)
+{
+  static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");
+  if (world_ < 2 || world_ > 8)
+    return fail(MPPIB_ERR_UNSUPPORTED, "peer-memory exchange is built for 2..8 ranks");
+  if (!p2p_gather_)
+  {
+    const size_t floats = (size_t)2 * world_ * D_ * pstride_ + 2 * world_ + 16;
+    CUDA_TRY(p2p_gather_.alloc(floats));
+    CUDA_TRY(cudaMemset(p2p_gather_, 0, floats * sizeof(float)));
+  }
+  cudaIpcMemHandle_t h;
+  CUDA_TRY(cudaIpcGetMemHandle(&h, p2p_gather_));
+  memcpy(handle_64, &h, 64);
+  return MPPIB_OK;
+}
+
+int Reduction::p2p_open(const void* handles)
+{
+  if (!p2p_gather_)
+    return fail(MPPIB_ERR_STATE, "call mppib_comm_p2p_handle first");
+  const size_t gather_floats = (size_t)2 * world_ * D_ * pstride_;
+  for (int r = 0; r < world_; r++)
+  {
+    float* base = nullptr;
+    if (r == rank_)
+      base = p2p_gather_;
+    else
+    {
+      cudaIpcMemHandle_t h;
+      memcpy(&h, (const char*)handles + (size_t)r * 64, 64);
+      void* p = nullptr;
+      cudaError_t rc = cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess);
+      if (rc != cudaSuccess)
+      {
+        cudaGetLastError();
+        return fail(MPPIB_ERR_CUDA, "cudaIpcOpenMemHandle(rank %d) failed: %s — keep the NCCL path", r,
+                    cudaGetErrorString(rc));
+      }
+      peer_opened_[r] = p;
+      base = (float*)p;
+    }
+    peers_.gather[r] = base;
+    peers_.flags[r] = reinterpret_cast<unsigned*>(base + gather_floats);
+  }
+  p2p_ = true;
+  p2p_opened_ = true;
+  return MPPIB_OK;
+}
+
+int Reduction::set_p2p(bool on)
+{
+  if (on && !p2p_opened_)
+    return fail(MPPIB_ERR_STATE, "mppib_comm_p2p_open has not succeeded on this rank");
+  if (!on && !comm_)
+    return fail(MPPIB_ERR_STATE, "no NCCL communicator to fall back to (mppib_comm_init)");
+  p2p_ = on;
+  return MPPIB_OK;
 }
 
 static int check_ready(mppib_engine* e)
@@ -634,26 +734,9 @@ static int check_ready(mppib_engine* e)
     return fail(MPPIB_ERR_STATE, "MPPIB_BLOB_COSTMAP not set");
   if (e->desc.dynamics_id == MPPIB_DYN_RACER_LSTM && !e->have_lstm)
     return fail(MPPIB_ERR_STATE, "MPPIB_BLOB_LSTM_WEIGHTS not set");
-  if (e->desc.world_size > 1 && !e->comm)
+  if (!e->reduction.ready())
     return fail(MPPIB_ERR_STATE, "world_size > 1 but mppib_comm_init was not called");
   return MPPIB_OK;
-}
-
-static void read_result(mppib_engine& e, float* U_out, mppib_solve_stats* stats)
-{
-  for (int d = 0; d < e.D; d++)
-  {
-    const float* r = e.result_h + (size_t)d * e.pstride;
-    if (stats)
-    {
-      stats[d].baseline = r[0];
-      stats[d].normalizer = r[1];
-      stats[d].sum_w2 = r[2];
-      stats[d].pad = 0.0f;
-    }
-    if (U_out)
-      memcpy(U_out + (size_t)d * e.TC, r + kPartialHeader, sizeof(float) * e.TC);
-  }
 }
 
 // ---- choice of the rollout kernel (K1) ----------------------------------------------------------------------------
@@ -1079,11 +1162,6 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (e->rmppi && desc->num_distributions != 2)
     return fail(MPPIB_ERR_INVALID_ARG, "MPPIB_FLAG_RMPPI needs num_distributions == 2 (nominal, real)");
   e->writeback = e->rmppi || (desc->flags & MPPIB_FLAG_WRITEBACK_CONTROLS) != 0;
-  e->use_pdl = !getenv("MPPIB_NO_PDL");
-  e->mapped_result = !getenv("MPPIB_NO_MAPPED_RESULT");
-  // polling a mapped flag was not found faster than cudaStreamSynchronize and costs K2 two system fences; off unless
-  // MPPIB_SPIN_WAIT is set
-  e->spin_wait = e->mapped_result && getenv("MPPIB_SPIN_WAIT") != nullptr;
 
   if (e->D * e->TC > kMaxMeanFloats)
     return fail(MPPIB_ERR_UNSUPPORTED, "D*T*C = %d exceeds %d", e->D * e->TC, kMaxMeanFloats);
@@ -1103,7 +1181,6 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return rc;
   if (e->k1.stream_readback)
     e->writeback = true;
-  e->pstride = ((kPartialHeader + e->TC + 3) / 4) * 4;
 
   int prio_lo = 0, prio_hi = 0;
   CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
@@ -1115,23 +1192,10 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (int rc = e->noise.create(e->desc, e->N, e->n_offset, e->n_local, e->T, e->C, e->num_sms, e->stream, prio_lo))
     return rc;
   CUDA_TRY(e->costs_d.alloc((size_t)e->D * e->n_local));
-  CUDA_TRY(e->partials_d.alloc((size_t)e->k1.grid * e->D * e->pstride));
-  CUDA_TRY(e->headers_d.alloc((size_t)e->k1.grid * e->D));
-  CUDA_TRY(e->result_d.alloc((size_t)e->D * e->pstride));
-  CUDA_TRY(e->result_h.alloc((size_t)e->D * e->pstride, cudaHostAllocMapped, &e->result_h_dev));
-  memset(e->result_h, 0, (size_t)e->D * e->pstride * sizeof(float));
-  CUDA_TRY(e->k2_counter_d.alloc(1));
-  CUDA_TRY(cudaMemsetAsync(e->k2_counter_d, 0, sizeof(unsigned), e->stream));
-  CUDA_TRY(e->done_flag_h.alloc(16, cudaHostAllocMapped, &e->done_flag_dev));  // 64 bytes
-  *e->done_flag_h = 0u;
+  if (int rc = e->reduction.create(e->D, e->TC, e->k1.grid, world, desc->rank, e->stream))
+    return rc;
   if (e->writeback)
     CUDA_TRY(e->controls_d.alloc((size_t)e->D * e->n_local * e->TC));
-  if (world > 1)
-  {
-    CUDA_TRY(e->rank_rec_d.alloc((size_t)e->D * e->pstride));
-    CUDA_TRY(e->gather_d.alloc((size_t)world * e->D * e->pstride));
-    CUDA_TRY(e->gather_hdr_d.alloc((size_t)world * e->D));
-  }
   for (int i = 0; i < 4; i++)
     CUDA_TRY(e->ev[i].create());
 
@@ -1146,18 +1210,14 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   return MPPIB_OK;
 }
 
-// What must go before the members release themselves: the stream drained, then what hangs on it. The members follow in
-// reverse order of declaration, the stream last (engine_internal.cuh); the noise source drains its own side stream.
+// What must go before the members release themselves: the stream drained. The members follow in reverse order of
+// declaration, the stream last (engine_internal.cuh); the noise source drains its own side stream, and the reduction
+// releases the communicator and the peer mappings.
 mppib_engine::~mppib_engine()
 {
   cudaSetDevice(desc.device);
   if (stream)
     cudaStreamSynchronize(stream);
-  if (comm && g_nccl.CommDestroy)
-    g_nccl.CommDestroy(comm);
-  for (int r = 0; r < 8; r++)
-    if (peer_opened[r])
-      cudaIpcCloseMemHandle(peer_opened[r]);
 }
 
 int mppib_destroy(mppib_engine* e)
@@ -1381,75 +1441,24 @@ int mppib_comm_init(mppib_engine* e, const void* unique_id_128)
 {
   if (!e || !unique_id_128)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (e->desc.world_size <= 1)
-    return MPPIB_OK;
-  if (!g_nccl.load())
-    return fail(MPPIB_ERR_NCCL, "libnccl.so.2 could not be loaded: %s", dlerror());
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  NcclUniqueId id;
-  memcpy(&id, unique_id_128, sizeof(id));
-  int rc = g_nccl.CommInitRank(&e->comm, e->desc.world_size, id, e->desc.rank);
-  if (rc != 0)
-    return fail(MPPIB_ERR_NCCL, "ncclCommInitRank failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "?");
-  return MPPIB_OK;
+  return e->reduction.comm_init(unique_id_128);
 }
 
 int mppib_comm_p2p_handle(mppib_engine* e, void* handle_64)
 {
   if (!e || !handle_64)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");
-  const int world = e->desc.world_size;
-  if (world < 2 || world > 8)
-    return fail(MPPIB_ERR_UNSUPPORTED, "peer-memory exchange is built for 2..8 ranks");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  if (!e->p2p_gather_d)
-  {
-    const size_t floats = (size_t)2 * world * e->D * e->pstride + 2 * world + 16;
-    CUDA_TRY(e->p2p_gather_d.alloc(floats));
-    CUDA_TRY(cudaMemset(e->p2p_gather_d, 0, floats * sizeof(float)));
-  }
-  cudaIpcMemHandle_t h;
-  CUDA_TRY(cudaIpcGetMemHandle(&h, e->p2p_gather_d));
-  memcpy(handle_64, &h, 64);
-  return MPPIB_OK;
+  return e->reduction.p2p_handle(handle_64);
 }
 
 int mppib_comm_p2p_open(mppib_engine* e, const void* handles)
 {
   if (!e || !handles)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (!e->p2p_gather_d)
-    return fail(MPPIB_ERR_STATE, "call mppib_comm_p2p_handle first");
-  const int world = e->desc.world_size;
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  const size_t gather_floats = (size_t)2 * world * e->D * e->pstride;
-  for (int r = 0; r < world; r++)
-  {
-    float* base = nullptr;
-    if (r == e->desc.rank)
-      base = e->p2p_gather_d;
-    else
-    {
-      cudaIpcMemHandle_t h;
-      memcpy(&h, (const char*)handles + (size_t)r * 64, 64);
-      void* p = nullptr;
-      cudaError_t rc = cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess);
-      if (rc != cudaSuccess)
-      {
-        cudaGetLastError();
-        return fail(MPPIB_ERR_CUDA, "cudaIpcOpenMemHandle(rank %d) failed: %s — keep the NCCL path", r,
-                    cudaGetErrorString(rc));
-      }
-      e->peer_opened[r] = p;
-      base = (float*)p;
-    }
-    e->peers.gather[r] = base;
-    e->peers.flags[r] = reinterpret_cast<unsigned*>(base + gather_floats);
-  }
-  e->p2p = true;
-  e->p2p_opened = true;
-  return MPPIB_OK;
+  return e->reduction.p2p_open(handles);
 }
 
 int mppib_set_noise(mppib_engine* e, const float* host_eps, size_t count)
@@ -1500,11 +1509,11 @@ int mppib_reduce_only(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
   if (!e->solved_once)
     return fail(MPPIB_ERR_STATE, "no rollout has been run yet");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = launch_combine(*e, false);
+  rc = e->reduction.enqueue(false, e->costs_d, e->controls_d, e->n_local, e->lambda);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
-  read_result(*e, U_out, stats);
+  e->reduction.read(U_out, stats);
   return MPPIB_OK;
 }
 
@@ -1528,7 +1537,8 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
     return rc;
   if (e->timing)
     CUDA_TRY(cudaEventRecord(e->ev[2], e->stream));
-  rc = launch_combine(*e, /*after_k1=*/!e->timing);  // timing mode records an event between K1 and K2: no PDL then
+  // timing mode records an event between K1 and K2: no PDL then
+  rc = e->reduction.enqueue(/*after_k1=*/!e->timing, e->costs_d, e->controls_d, e->n_local, e->lambda);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(e->noise.read_by_kernel());  // K1 read it; recorded after K2, so nothing sits between K1 and PDL's K2
@@ -1538,43 +1548,9 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
   return MPPIB_OK;
 }
 
-// Blocks until the last enqueued solve is complete. Fast path: poll the mapped word K2's last block writes after the
-// result record (the record travels the same way, so it is visible when the flag is); every few thousand polls the
-// stream is queried so that a failed launch cannot spin forever, and timing mode uses a full synchronize (events).
-static int wait_for_stream(mppib_engine* e)
-{
-  if (e->spin_wait && !e->timing && e->flag_armed && e->solve_seq != 0)
-  {
-    const unsigned want = e->solve_seq;
-    for (unsigned spins = 1;; spins++)
-    {
-      if (*e->done_flag_h == want)
-        return MPPIB_OK;
-      if ((spins & 0x3fff) == 0)
-      {
-        cudaError_t q = cudaStreamQuery(e->stream);
-        if (q == cudaSuccess)
-          break;  // stream drained (the flag write is then visible as well)
-        if (q != cudaErrorNotReady)
-        {
-          cudaGetLastError();
-          return fail(MPPIB_ERR_CUDA, "solve failed: %s", cudaGetErrorString(q));
-        }
-      }
-#if defined(__x86_64__)
-      __builtin_ia32_pause();
-#endif
-    }
-  }
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
-}
-
 static int wait_solve(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
 {
-  int rcw = wait_for_stream(e);
-  if (rcw != MPPIB_OK)
-    return rcw;
+  CUDA_TRY(cudaStreamSynchronize(e->stream));
   e->pending = 0;
   e->timing_valid = e->timing;
   if (e->timing)
@@ -1591,7 +1567,7 @@ static int wait_solve(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
     }
   }
   e->solved_once = true;
-  read_result(*e, U_out, stats);
+  e->reduction.read(U_out, stats);
   return MPPIB_OK;
 }
 
@@ -1680,19 +1656,7 @@ int mppib_set_tsallis(mppib_engine* e, float gamma, float r)
 {
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
-  if (gamma != 0.0f && r != 0.0f)
-  {
-    if (!e->controls_d)
-      return fail(MPPIB_ERR_STATE, "Tsallis weights reduce the written-back controls: create the engine with "
-                                   "MPPIB_FLAG_WRITEBACK_CONTROLS");
-    if (e->desc.world_size != 1)
-      return fail(MPPIB_ERR_UNSUPPORTED, "Tsallis weights are built for one rank");
-    if (r == 1.0f || !(gamma > 0.0f))
-      return fail(MPPIB_ERR_INVALID_ARG, "Tsallis weights need gamma > 0 and r != 1");
-  }
-  e->tsallis_gamma = gamma;
-  e->tsallis_r = r;
-  return MPPIB_OK;
+  return e->reduction.set_tsallis(gamma, r, e->controls_d != nullptr);
 }
 
 int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* feedback_gains)
@@ -1919,8 +1883,8 @@ int mppib_nominal_trajectory(mppib_engine* e, const float* x0, const float* U, c
     CUDA_TRY(e->nom_d.alloc(n_u + n_s + n_o));
   if (!e->nom_h)
     CUDA_TRY(e->nom_h.alloc(n_u + n_s + n_o, cudaHostAllocDefault));
-  const float* u_src = e->result_d + kPartialHeader;  // the optimised sequence where K2 / KX left it
-  int u_stride = e->pstride;
+  const float* u_src = e->reduction.result() + kPartialHeader;  // the optimised sequence where K2 / KX left it
+  int u_stride = e->reduction.pstride();
   if (U)
   {
     if (!e->nom_u_d)
@@ -1944,14 +1908,7 @@ int mppib_nominal_trajectory(mppib_engine* e, const float* x0, const float* U, c
 int mppib_set_option(mppib_engine* e, int option, long long value)
 {
   if (e && option == MPPIB_OPT_P2P_ENABLE)
-  {
-    if (value != 0 && !e->p2p_opened)
-      return fail(MPPIB_ERR_STATE, "mppib_comm_p2p_open has not succeeded on this rank");
-    if (value == 0 && !e->comm)
-      return fail(MPPIB_ERR_STATE, "no NCCL communicator to fall back to (mppib_comm_init)");
-    e->p2p = value != 0;
-    return MPPIB_OK;
-  }
+    return e->reduction.set_p2p(value != 0);
   if (e && option == MPPIB_OPT_COLORED_OFFSET_T)
     return e->noise.set_offset_t(value);
   if (!e)
@@ -2015,7 +1972,7 @@ int mppib_get_weights(mppib_engine* e, float* host_weights)
   if (!e->weights_d)
     CUDA_TRY(e->weights_d.alloc(n));
   const dim3 grid((e->n_local + 255) / 256 > 1024 ? 1024 : (e->n_local + 255) / 256, e->D);
-  weights_kernel<<<grid, 256, 0, e->stream>>>(e->costs_d, e->result_d, e->n_local, e->pstride,
+  weights_kernel<<<grid, 256, 0, e->stream>>>(e->costs_d, e->reduction.result(), e->n_local, e->reduction.pstride(),
                                               (float)(1.0 / e->lambda), e->weights_d);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(host_weights, e->weights_d, n * sizeof(float), cudaMemcpyDeviceToHost, e->stream));

@@ -10,6 +10,9 @@
  * revision (kEngineAbi is checked at registration).
  * An engine keeps a pointer to its pair's entry and one K1Plan: the form and geometry of its rollout kernel, chosen once
  * by engine.cu's choose_k1. Pair<>::kernel maps the plan's form to the instantiation that launches.
+ * Two parts of a solve have an owner of their own, declared in their headers and defined in engine.cu: the noise draw
+ * (NoiseSource, noise_source.cuh) and the merge from K1's block partials to the result record (Reduction, reduction.cuh);
+ * K1 reads the current noise buffer and writes the partials through their accessors.
  */
 #pragma once
 #include <cuda.h>
@@ -33,6 +36,7 @@
 #include "noise_source.cuh"
 #include "plugins/costs.cuh"
 #include "plugins/dynamics.cuh"
+#include "reduction.cuh"
 #include "rollout_kernel.cuh"
 #include "rollout_kernel_ar_ws.cuh"
 #include "rollout_kernel_nn_tc.cuh"
@@ -63,7 +67,6 @@ static inline int fail(int status, const char* fmt, A... a)
       return fail(MPPIB_ERR_CURAND, "%s failed: curandStatus %d (%s:%d)", #expr, (int)_s, __FILE__, __LINE__);         \
   } while (0)
 
-typedef struct ncclComm* ncclComm_t;
 using namespace mppib;
 
 // ---- K1's form and geometry, chosen once per engine by mppib_create (engine.cu: choose_k1) ------------------------
@@ -112,19 +115,10 @@ struct mppib_engine
   int S = 0, C = 0, O = 0, D = 1;
   int N = 0, T = 0, TC = 0;
   int n_local = 0, n_offset = 0;
-  int pstride = 0, nchunks = 0;
+  int nchunks = 0;
   int num_sms = 0;  // multiprocessors of the device (grid-stride kernels launch up to 16 CTAs per SM)
-  bool use_pdl = true;
-  bool mapped_result = true;  // K2 writes the result record straight into mapped pinned host memory
-  bool spin_wait = true;      // the host waits for the solve by polling a mapped flag K2's last block sets
-  DeviceBuffer<unsigned> k2_counter_d;
-  PinnedBuffer<volatile unsigned> done_flag_h;
-  volatile unsigned* done_flag_dev = nullptr;  // device alias of done_flag_h
-  unsigned solve_seq = 0;
-  bool flag_armed = false;  // the LAST enqueued solve ends in a kernel that publishes done_flag == solve_seq
   bool writeback = false;
   bool rmppi = false;  // MPPIB_FLAG_RMPPI
-  float tsallis_gamma = 0.0f, tsallis_r = 0.0f;  // both non-zero: Tsallis weights (mppib_set_tsallis)
   float value_func_threshold = 1000.0f;  // robust_mppi_controller.cuh default
   DeviceBuffer<float> fb_gains_d;        // [T][S][C] or null
   DeviceBuffer<float> eval_states_d;     // init-eval scratch: candidates, strides, costs
@@ -170,15 +164,7 @@ struct mppib_engine
 
   // device buffers
   DeviceBuffer<float> costs_d;        // [D][n_local]
-  DeviceBuffer<float> partials_d;     // [grid][D][pstride]
-  DeviceBuffer<float4> headers_d;     // [grid][D] compact (beta, eta, sum w^2)
-  DeviceBuffer<float4> gather_hdr_d;  // [world][D]
   DeviceBuffer<float> controls_d;     // optional [D][n_local][T][C]
-  DeviceBuffer<float> rank_rec_d;     // [D][pstride] this rank's record (world > 1)
-  DeviceBuffer<float> gather_d;       // [world][D][pstride]
-  DeviceBuffer<float> result_d;       // [D][pstride] final record (device copy)
-  PinnedBuffer<float> result_h;       // mapped pinned host copy K2 writes directly
-  float* result_h_dev = nullptr;      // device alias of result_h
   DeviceBuffer<float> weights_d;      // lazily allocated for mppib_get_weights
   DeviceBuffer<unsigned char> l2_flush_d;  // optional: all of it is written between K0 and K1 to evict the noise from L2
   int pending = 0;               // solves enqueued and not yet waited for
@@ -188,15 +174,8 @@ struct mppib_engine
 
   CUtensorMap tmap[2]{};  // K1's TMA view of noise.buffer(i) (its box is K1's block width)
 
-  // comm
-  ncclComm_t comm = nullptr;
-  // peer-memory exchange (combine_kernel.cuh: exchange_merge_kernel)
-  bool p2p = false;
-  bool p2p_opened = false;
-  DeviceBuffer<float> p2p_gather_d;  // [2][world][D][pstride] followed by the flag words [2][world]
-  PeerTable peers{};
-  void* peer_opened[8] = { nullptr };
-  unsigned p2p_seq = 0;
+  // K1's block partials, K2 and the cross-rank merge, the result record, Tsallis weights, NCCL and KX (reduction.cuh)
+  Reduction reduction;
 
   // timing
   bool timing = false;
@@ -370,14 +349,14 @@ struct Pair
     fill_pair_args(a, e, iter);
     a.eps = e.noise.eps();
     a.costs = e.costs_d;
-    a.partials = e.partials_d;
-    a.headers = e.headers_d;
+    a.partials = e.reduction.partials();
+    a.headers = e.reduction.headers();
     a.controls_out = e.writeback ? e.controls_d.get() : nullptr;
     a.n_local = e.n_local;
     a.n_offset = e.n_offset;
     a.T = e.T;
     a.nchunks = e.nchunks;
-    a.pstride = e.pstride;
+    a.pstride = e.reduction.pstride();
     a.opt_stride = opt_stride;
     a.use_tma = e.k1.use_tma ? 1 : 0;
     a.dyn_shared_floats = e.k1.dyn_shared_floats;
