@@ -10,9 +10,10 @@
  * revision (kEngineAbi is checked at registration).
  * An engine keeps a pointer to its pair's entry and one K1Plan: the form and geometry of its rollout kernel, chosen once
  * by engine.cu's choose_k1. Pair<>::kernel maps the plan's form to the instantiation that launches.
- * Two parts of a solve have an owner of their own, declared in their headers and defined in engine.cu: the noise draw
- * (NoiseSource, noise_source.cuh) and the merge from K1's block partials to the result record (Reduction, reduction.cuh);
- * K1 reads the current noise buffer and writes the partials through their accessors.
+ * Three parts of the engine have an owner of their own, declared in their headers and defined in engine.cu: the noise
+ * draw (NoiseSource, noise_source.cuh), the merge from K1's block partials to the result record (Reduction,
+ * reduction.cuh) and the model's blobs: parameters, weights and maps (ModelParams, model_params.cuh). K1 reads the
+ * current noise buffer, writes the partials and takes the model's blobs through their accessors.
  */
 #pragma once
 #include <cuda.h>
@@ -33,6 +34,7 @@
 #include "combine_kernel.cuh"
 #include "ddp_kernel.cuh"
 #include "device_resources.cuh"
+#include "model_params.cuh"
 #include "noise_source.cuh"
 #include "plugins/costs.cuh"
 #include "plugins/dynamics.cuh"
@@ -143,23 +145,7 @@ struct mppib_engine
   // solver scalars
   float dt = 0.01f, lambda = 1.0f, alpha = 0.0f;
 
-  // parameter blobs (host copies)
-  std::vector<unsigned char> dyn_blob, cost_blob;
-  bool have_dyn = false, have_cost = false;  // the sampler's parameters are noise.params()
-
-  // aux device resources
-  DeviceBuffer<float> nn_theta_d;
-  DeviceBuffer<float> lstm_theta_d;  // MPPIB_BLOB_LSTM_WEIGHTS
-  bool have_lstm = false;
-  DeviceBuffer<float> elev_d;            // MPPIB_BLOB_ELEVATION_MAP: width * height floats, row-major
-  // host copies of the weight / map blobs for mppib_compute_control's host tail (the library's host twins)
-  std::vector<float> nn_theta_h, lstm_theta_h;
-  std::vector<unsigned char> elev_h;
-  mppib_elevation_map_header elev_hdr{};  // use == 0 until a map is set
-  DeviceBuffer<float> cost_tex_d;            // MPPIB_BLOB_COST_TEXTURE: QuadrotorMapCost's map, width * height floats
-  mppib_elevation_map_header cost_tex_hdr{};  // use == 0 until a map is set
-  ArrayTexture costmap_tex;                   // MPPIB_BLOB_COSTMAP: float4 array + its texture object
-
+  ModelParams model;  // the dynamics and cost blobs, weights and maps (model_params.cuh)
   NoiseSource noise;  // K0 / K0c / NLN draw, its sampler parameters, two buffers and prefetch (noise_source.cuh)
 
   // device buffers
@@ -189,50 +175,43 @@ struct mppib_engine
 template <class AUX>
 struct AuxFill
 {
-  static void fill(AUX&, const mppib_engine&)
+  static void fill(AUX&, const ModelParams&)
   {
   }
 };
 template <>
 struct AuxFill<plugins::AutorallyNNDynamics::Aux>
 {
-  static void fill(plugins::AutorallyNNDynamics::Aux& a, const mppib_engine& e)
+  static void fill(plugins::AutorallyNNDynamics::Aux& a, const ModelParams& m)
   {
-    a.theta_d = e.nn_theta_d;
+    a.theta_d = m.nn_weights();
   }
 };
 template <>
 struct AuxFill<plugins::RacerLSTMDynamics::Aux>
 {
-  static void fill(plugins::RacerLSTMDynamics::Aux& a, const mppib_engine& e)
+  static void fill(plugins::RacerLSTMDynamics::Aux& a, const ModelParams& m)
   {
-    a.theta_d = e.lstm_theta_d;
-    a.H = e.desc.model_dims[0];
-    a.L1 = e.desc.model_dims[1];
-    a.elev.data = e.elev_d;
-    a.elev.hdr = e.elev_hdr;
-    if (!e.elev_d)
-      a.elev.hdr.use = 0;
+    a.theta_d = m.lstm_weights();
+    a.H = m.dims()[0];
+    a.L1 = m.dims()[1];
+    a.elev = m.elevation_map();
   }
 };
 template <>
 struct AuxFill<plugins::ARStandardCost::Aux>
 {
-  static void fill(plugins::ARStandardCost::Aux& a, const mppib_engine& e)
+  static void fill(plugins::ARStandardCost::Aux& a, const ModelParams& m)
   {
-    a.costmap_tex = e.costmap_tex;
+    a.costmap_tex = m.costmap();
   }
 };
-
 template <>
 struct AuxFill<plugins::QuadrotorMapCost::Aux>
 {
-  static void fill(plugins::QuadrotorMapCost::Aux& a, const mppib_engine& e)
+  static void fill(plugins::QuadrotorMapCost::Aux& a, const ModelParams& m)
   {
-    a.map.data = e.cost_tex_d;
-    a.map.hdr = e.cost_tex_hdr;
-    if (!e.cost_tex_d)
-      a.map.hdr.use = 0;
+    a.map = m.cost_texture();
   }
 };
 
@@ -240,8 +219,8 @@ struct AuxFill<plugins::QuadrotorMapCost::Aux>
 template <class P, class AUX>
 static void fill_dyn_args(P& dyn, AUX& aux, const mppib_engine& e)
 {
-  memcpy(&dyn, e.dyn_blob.data(), sizeof(dyn));
-  AuxFill<AUX>::fill(aux, e);
+  memcpy(&dyn, e.model.dyn(), sizeof(dyn));
+  AuxFill<AUX>::fill(aux, e.model);
 }
 // ... and the cost's, the solver scalars, and the sampler at optimisation iteration `iter` (std_dev_decay^iter,
 // gaussian.cu:423)
@@ -252,8 +231,8 @@ static void fill_pair_args(A& a, const mppib_engine& e, int iter)
   a.dt = e.dt;
   a.lambda = e.lambda;
   a.alpha = e.alpha;
-  memcpy(&a.cost, e.cost_blob.data(), sizeof(a.cost));
-  AuxFill<decltype(a.cost_aux)>::fill(a.cost_aux, e);
+  memcpy(&a.cost, e.model.cost(), sizeof(a.cost));
+  AuxFill<decltype(a.cost_aux)>::fill(a.cost_aux, e.model);
   const mppib_gaussian_params& sampler = e.noise.params();
   const float decay = powf(sampler.std_dev_decay, (float)iter);
   for (int d = 0; d < MPPIB_MAX_DISTRIBUTIONS; d++)

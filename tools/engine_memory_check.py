@@ -4,8 +4,10 @@ demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
     cost map replaced by one with four times the cells, the feedback gains set, freed and set again, a solve after each;
   - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time;
   - a ColoredNoise and an NLN engine (the samplers whose spectrum, plan and log-normal planes the noise source owns): solve,
-    new sampler parameters, solve, burn_draws, solve.
-The free device memory (cudaMemGetInfo) after all four are destroyed is compared with the value before they were created. The
+    new sampler parameters, solve, burn_draws, solve;
+  - an Autorally engine: solve, new NN weights, solve, a costmap with four times the texels, solve;
+  - a RACER LSTM engine: solve, new LSTM weights, solve, an elevation map with four times the cells, solve.
+The free device memory (cudaMemGetInfo) after all six are destroyed is compared with the value before they were created. The
 sequence runs twice and the second pass is the one checked: the first also loads the kernels, which stay on the device.
 Every call raises on a status other than MPPIB_OK. Prints one JSON line; exits 1 if the second pass leaves more than
 `--slack-mib` less free memory than it found (another process on a shared card can move the figure as well).
@@ -71,6 +73,32 @@ def exercise():
         e.burn_draws(3)
         e.solve(w.x0, w.U0)
         e.close()
+
+    # the model's weights and maps (csrc/model_params.cuh), each replaced between solves; the maps grow
+    w = W.autorally(1024, 40)
+    e = w.make_engine()
+    e.solve(w.x0, w.U0)
+    w.dyn.updateModel([6, 32, 32, 4], W.synthetic_nn_weights(5))
+    e.push_params()
+    e.solve(w.x0, w.U0)
+    ch0, xb, yb, ppm = W.track_map_standard()
+    w.cost.loadTrackData(np.kron(ch0, np.ones((2, 2), np.float32)), xb[0], xb[1], yb[0], yb[1], 2 * ppm)
+    e.push_params()
+    e.solve(w.x0, w.U0)
+    e.close()
+
+    w = W.racer_lstm_gaussian(1024, 40)
+    hills = lambda n: np.sin(0.3 * np.arange(n * n, dtype=np.float32)).reshape(n, n)  # noqa: E731
+    w.dyn.setElevationMap(hills(48), 0.5, (-12.0, -12.0, 0.0))
+    e = w.make_engine()
+    e.solve(w.x0, w.U0)
+    w.dyn.setAllValues(*W.synthetic_lstm_weights(4, 20, 9))
+    e.push_params()
+    e.solve(w.x0, w.U0)
+    w.dyn.setElevationMap(hills(96), 0.25, (-12.0, -12.0, 0.0))
+    e.push_params()
+    e.solve(w.x0, w.U0)
+    e.close()
 
 
 def main():
