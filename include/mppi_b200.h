@@ -186,7 +186,8 @@ typedef struct mppib_timing
   int samples;      /* synchronous solves averaged */
 } mppib_timing;
 /* Enable CUDA-event timestamps around each stage of subsequent solves (adds ~us; off by default); mppib_get_timing
- * returns the averages over the synchronous solves since the last enable call. */
+ * returns the averages since the last enable call over the solves enqueued while timing was on, each counted when it is
+ * waited for with timing still on (with several solves in flight, only the last). */
 int mppib_enable_timing(mppib_engine* e, int enable);
 int mppib_get_timing(mppib_engine* e, mppib_timing* out);
 /* Launch geometry actually used by K1 (for bench.py / DESIGN.md). */

@@ -1180,6 +1180,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     CUDA_TRY(e->stream.create(cudaStreamNonBlocking, prio_hi));
 
   e->model.create(e->desc, entry->dyn_bytes, entry->cost_bytes, e->stream);
+  e->feedback.create(e->S, e->C, e->T, e->stream);
   if (int rc = e->noise.create(e->desc, e->N, e->n_offset, e->n_local, e->T, e->C, e->num_sms, e->stream, prio_lo))
     return rc;
   CUDA_TRY(e->costs_d.alloc((size_t)e->D * e->n_local));
@@ -1187,8 +1188,7 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return rc;
   if (e->writeback)
     CUDA_TRY(e->controls_d.alloc((size_t)e->D * e->n_local * e->TC));
-  for (int i = 0; i < 4; i++)
-    CUDA_TRY(e->ev[i].create());
+  CUDA_TRY(e->timer.create());
 
   if (e->k1.use_tma)
     for (int i = 0; i < 2; i++)
@@ -1577,33 +1577,77 @@ int mppib_reduce_only(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
   return MPPIB_OK;
 }
 
+// ---- stage timing (engine_internal.cuh) -------------------------------------------------------------------------------
+cudaError_t StageTimer::create()
+{
+  for (Event& ev : ev_)
+    if (cudaError_t rc = ev.create())
+      return rc;
+  return cudaSuccess;
+}
+
+void StageTimer::enable(bool on)
+{
+  on_ = on;
+  for (double& s : sum_ms_)
+    s = 0.0;
+  n_ = 0;
+}
+
+void StageTimer::collect()
+{
+  if (!timed_ || !on_)
+    return;
+  timed_ = false;  // counted once
+  float ms[4];
+  if (cudaEventElapsedTime(&ms[0], ev_[0], ev_[1]) != cudaSuccess ||
+      cudaEventElapsedTime(&ms[1], ev_[1], ev_[2]) != cudaSuccess ||
+      cudaEventElapsedTime(&ms[2], ev_[2], ev_[3]) != cudaSuccess ||
+      cudaEventElapsedTime(&ms[3], ev_[0], ev_[3]) != cudaSuccess)
+  {
+    cudaGetLastError();  // leave no error behind for the next launch's check
+    return;
+  }
+  for (int i = 0; i < 4; i++)
+    sum_ms_[i] += ms[i];
+  n_++;
+}
+
+int StageTimer::read(mppib_timing* out) const
+{
+  if (n_ == 0)
+    return fail(MPPIB_ERR_STATE, "timing not enabled or no synchronous solve since it was enabled");
+  out->noise_ms = (float)(sum_ms_[0] / n_);
+  out->rollout_ms = (float)(sum_ms_[1] / n_);
+  out->reduce_ms = (float)(sum_ms_[2] / n_);
+  out->total_ms = (float)(sum_ms_[3] / n_);
+  out->samples = (int)n_;
+  return MPPIB_OK;
+}
+
 static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, int optimization_stride,
                          int iteration_num)
 {
-  if (e->timing)
-    CUDA_TRY(cudaEventRecord(e->ev[0], e->stream));
+  CUDA_TRY(e->timer.start(e->stream));
   int rc = e->noise.draw(optimization_stride);
   if (rc != MPPIB_OK)
     return rc;
   if (e->l2_flush_d)
     CUDA_TRY(cudaMemsetAsync(e->l2_flush_d, 0, e->l2_flush_d.capacity(), e->stream));
-  if (e->timing)
-    CUDA_TRY(cudaEventRecord(e->ev[1], e->stream));
+  CUDA_TRY(e->timer.mark(1, e->stream));
   rc = e->pair->launch(*e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   rc = e->noise.prefetch();
   if (rc != MPPIB_OK)
     return rc;
-  if (e->timing)
-    CUDA_TRY(cudaEventRecord(e->ev[2], e->stream));
-  // timing mode records an event between K1 and K2: no PDL then
-  rc = e->reduction.enqueue(/*after_k1=*/!e->timing, e->costs_d, e->controls_d, e->n_local, e->lambda);
+  CUDA_TRY(e->timer.mark(2, e->stream));
+  // a timed solve records an event between K1 and K2: no PDL then
+  rc = e->reduction.enqueue(/*after_k1=*/!e->timer.timed(), e->costs_d, e->controls_d, e->n_local, e->lambda);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(e->noise.read_by_kernel());  // K1 read it; recorded after K2, so nothing sits between K1 and PDL's K2
-  if (e->timing)
-    CUDA_TRY(cudaEventRecord(e->ev[3], e->stream));
+  CUDA_TRY(e->timer.mark(3, e->stream));
   e->pending++;
   return MPPIB_OK;
 }
@@ -1612,20 +1656,7 @@ static int wait_solve(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
 {
   CUDA_TRY(cudaStreamSynchronize(e->stream));
   e->pending = 0;
-  e->timing_valid = e->timing;
-  if (e->timing)
-  {
-    float ms[4];
-    if (cudaEventElapsedTime(&ms[0], e->ev[0], e->ev[1]) == cudaSuccess &&
-        cudaEventElapsedTime(&ms[1], e->ev[1], e->ev[2]) == cudaSuccess &&
-        cudaEventElapsedTime(&ms[2], e->ev[2], e->ev[3]) == cudaSuccess &&
-        cudaEventElapsedTime(&ms[3], e->ev[0], e->ev[3]) == cudaSuccess)
-    {
-      for (int i = 0; i < 4; i++)
-        e->acc_ms[i] += ms[i];
-      e->acc_n++;
-    }
-  }
+  e->timer.collect();
   e->solved_once = true;
   e->reduction.read(U_out, stats);
   return MPPIB_OK;
@@ -1710,6 +1741,104 @@ int mppib_set_tsallis(mppib_engine* e, float gamma, float r)
   return e->reduction.set_tsallis(gamma, r, e->controls_d != nullptr);
 }
 
+// ---- the feedback controller (feedback.cuh) ---------------------------------------------------------------------------
+void Feedback::create(int S, int C, int T, cudaStream_t stream)
+{
+  S_ = S;
+  C_ = C;
+  T_ = T;
+  stream_ = stream;
+  Q_.assign((size_t)S * S, 0.0f);
+  R_.assign((size_t)C * C, 0.0f);
+  for (int i = 0; i < S; i++)
+    Q_[(size_t)i * (S + 1)] = 1.0f;
+  for (int i = 0; i < C; i++)
+    R_[(size_t)i * (C + 1)] = 1.0f;
+  Qf_ = Q_;
+}
+
+int Feedback::set_weights(const float* Q, const float* Q_f, const float* R, int iters)
+{
+  if (iters < 1)
+    return fail(MPPIB_ERR_INVALID_ARG, "num_iterations must be >= 1 (got %d)", iters);
+  for (int i = 0; i < S_ * S_; i++)
+    if (!std::isfinite(Q[i]) || !std::isfinite(Q_f[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight Q / Q_f entry %d is not finite", i);
+  for (int i = 0; i < C_ * C_; i++)
+    if (!std::isfinite(R[i]))
+      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight R entry %d is not finite", i);
+  Q_.assign(Q, Q + S_ * S_);
+  Qf_.assign(Q_f, Q_f + S_ * S_);
+  R_.assign(R, R + C_ * C_);
+  iters_ = iters;
+  return MPPIB_OK;
+}
+
+// The gains are read by the K1 of a solve still in flight, so they are freed only once the stream has drained; a new
+// trajectory is copied in stream order, after that K1.
+int Feedback::set_rmppi(float threshold, const float* host_gains)
+{
+  threshold_ = threshold;
+  const size_t n = (size_t)T_ * S_ * C_;
+  if (host_gains)
+  {
+    for (size_t i = 0; i < n; i++)
+      if (!std::isfinite(host_gains[i]))
+        return fail(MPPIB_ERR_INVALID_ARG, "feedback gain %zu is not finite", i);
+    gains_set_ = false;  // the device copy changes from here on
+    if (!gains_)
+      CUDA_TRY(gains_.alloc(n));
+    CUDA_TRY(cudaMemcpyAsync(gains_, host_gains, n * sizeof(float), cudaMemcpyHostToDevice, stream_));
+    CUDA_TRY(cudaStreamSynchronize(stream_));
+    gains_set_ = true;
+  }
+  else if (gains_)
+  {
+    gains_set_ = false;
+    CUDA_TRY(cudaStreamSynchronize(stream_));
+    gains_.reset();
+  }
+  return MPPIB_OK;
+}
+
+int Feedback::compute(mppib_engine& e, int T, const float* x0, const float* x_target, const float* u_target, bool to_rmppi,
+                      float* gains, float* x_out, float* u_out, float* jac_out)
+{
+  const ddp::WsLayout L = ddp::ws_layout(T, S_, C_);
+  CUDA_TRY(ws_.reserve(L.total, stream_));
+  if (!status_)
+    CUDA_TRY(status_.alloc(1));
+  if (to_rmppi && !gains_)
+    CUDA_TRY(gains_.alloc((size_t)T * S_ * C_));
+  float* ws = ws_;
+  CUDA_TRY(cudaMemcpyAsync(ws + L.xt, x_target, (size_t)T * S_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
+  // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
+  CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
+  if (int rc = e.pair->ddp(e, T, x0, to_rmppi ? gains_.get() : nullptr))
+    return rc;
+  int status = 0;
+  CUDA_TRY(cudaMemcpyAsync(&status, status_, sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  if (status != 0)
+    return fail(MPPIB_ERR_INVALID_ARG, "DDP: the LDLT of Q_uu failed at step %d (the reference exits, ddp.h:112-116); "
+                                       "gains left unchanged", status - 1);
+  if (to_rmppi)
+    gains_set_ = true;  // the kernel has written the whole trajectory
+  if (gains)
+    CUDA_TRY(cudaMemcpyAsync(gains, ws + L.K, (size_t)T * S_ * C_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  if (x_out)
+    CUDA_TRY(cudaMemcpyAsync(x_out, ws + L.x, (size_t)T * S_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  if (u_out)
+    CUDA_TRY(cudaMemcpyAsync(u_out, ws + L.u, (size_t)T * C_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  if (jac_out)
+    CUDA_TRY(cudaMemcpyAsync(jac_out, ws + L.jac, (size_t)T * S_ * (S_ + C_) * sizeof(float), cudaMemcpyDeviceToHost,
+                             stream_));
+  if (gains || x_out || u_out || jac_out)
+    CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
+}
+
 int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* feedback_gains)
 {
   if (!e)
@@ -1717,44 +1846,14 @@ int mppib_set_rmppi(mppib_engine* e, float value_func_threshold, const float* fe
   if (!e->rmppi)
     return fail(MPPIB_ERR_STATE, "engine was not created with MPPIB_FLAG_RMPPI");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  e->value_func_threshold = value_func_threshold;
-  const size_t n = (size_t)e->T * e->S * e->C;
-  if (feedback_gains)
-  {
-    for (size_t i = 0; i < n; i++)
-      if (!std::isfinite(feedback_gains[i]))
-        return fail(MPPIB_ERR_INVALID_ARG, "feedback gain %zu is not finite", i);
-    if (!e->fb_gains_d)
-      CUDA_TRY(e->fb_gains_d.alloc(n));
-    CUDA_TRY(cudaMemcpyAsync(e->fb_gains_d, feedback_gains, n * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-  }
-  else if (e->fb_gains_d)
-  {
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    e->fb_gains_d.reset();
-  }
-  return MPPIB_OK;
+  return e->feedback.set_rmppi(value_func_threshold, feedback_gains);
 }
 
 int mppib_set_ddp(mppib_engine* e, const float* Q, const float* Q_f, const float* R, int num_iterations)
 {
   if (!e || !Q || !Q_f || !R)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (num_iterations < 1)
-    return fail(MPPIB_ERR_INVALID_ARG, "num_iterations must be >= 1 (got %d)", num_iterations);
-  const int S = e->S, C = e->C;
-  for (int i = 0; i < S * S; i++)
-    if (!std::isfinite(Q[i]) || !std::isfinite(Q_f[i]))
-      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight Q / Q_f entry %d is not finite", i);
-  for (int i = 0; i < C * C; i++)
-    if (!std::isfinite(R[i]))
-      return fail(MPPIB_ERR_INVALID_ARG, "DDP weight R entry %d is not finite", i);
-  e->ddp_Q.assign(Q, Q + S * S);
-  e->ddp_Qf.assign(Q_f, Q_f + S * S);
-  e->ddp_R.assign(R, R + C * C);
-  e->ddp_iters = num_iterations;
-  return MPPIB_OK;
+  return e->feedback.set_weights(Q, Q_f, R, num_iterations);
 }
 
 int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_target, const float* u_target, int to_rmppi,
@@ -1786,41 +1885,7 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
     if (!std::isfinite(u_target[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "u_target entry %zu is not finite", i);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  CUDA_TRY(e->ddp_ws_d.reserve(ddp::ws_layout(T, S, C).total, e->stream));
-  if (!e->ddp_status_d)
-    CUDA_TRY(e->ddp_status_d.alloc(1));
-  if (to_rmppi && !e->fb_gains_d)
-  {
-    CUDA_TRY(e->fb_gains_d.alloc((size_t)T * S * C));
-    CUDA_TRY(cudaMemsetAsync(e->fb_gains_d, 0, (size_t)T * S * C * sizeof(float), e->stream));
-  }
-  const ddp::WsLayout L = ddp::ws_layout(T, S, C);
-  float* ws = e->ddp_ws_d;
-  CUDA_TRY(cudaMemcpyAsync(ws + L.xt, x_target, (size_t)T * S * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
-  CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  int rc = e->pair->ddp(*e, T, x0, to_rmppi ? e->fb_gains_d.get() : nullptr);
-  if (rc != MPPIB_OK)
-    return rc;
-  int status = 0;
-  CUDA_TRY(cudaMemcpyAsync(&status, e->ddp_status_d, sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  if (status != 0)
-    return fail(MPPIB_ERR_INVALID_ARG, "DDP: the LDLT of Q_uu failed at step %d (the reference exits, ddp.h:112-116); "
-                                       "gains left unchanged", status - 1);
-  if (gains)
-    CUDA_TRY(cudaMemcpyAsync(gains, ws + L.K, (size_t)T * S * C * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  if (x_out)
-    CUDA_TRY(cudaMemcpyAsync(x_out, ws + L.x, (size_t)T * S * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  if (u_out)
-    CUDA_TRY(cudaMemcpyAsync(u_out, ws + L.u, (size_t)T * C * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  if (jac_out)
-    CUDA_TRY(cudaMemcpyAsync(jac_out, ws + L.jac, (size_t)T * S * (S + C) * sizeof(float), cudaMemcpyDeviceToHost,
-                             e->stream));
-  if (gains || x_out || u_out || jac_out)
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->feedback.compute(*e, T, x0, x_target, u_target, to_rmppi != 0, gains, x_out, u_out, jac_out);
 }
 
 int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides, int num_candidates,
@@ -2033,11 +2098,7 @@ int mppib_enable_timing(mppib_engine* e, int enable)
 {
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
-  e->timing = enable != 0;
-  e->timing_valid = false;
-  for (int i = 0; i < 4; i++)
-    e->acc_ms[i] = 0.0;
-  e->acc_n = 0;
+  e->timer.enable(enable != 0);
   return MPPIB_OK;
 }
 
@@ -2045,15 +2106,7 @@ int mppib_get_timing(mppib_engine* e, mppib_timing* out)
 {
   if (!e || !out)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (e->acc_n == 0)
-    return fail(MPPIB_ERR_STATE, "timing not enabled or no synchronous solve since it was enabled");
-  // averages over the synchronous solves since mppib_enable_timing(e, 1)
-  out->noise_ms = (float)(e->acc_ms[0] / e->acc_n);
-  out->rollout_ms = (float)(e->acc_ms[1] / e->acc_n);
-  out->reduce_ms = (float)(e->acc_ms[2] / e->acc_n);
-  out->total_ms = (float)(e->acc_ms[3] / e->acc_n);
-  out->samples = (int)e->acc_n;
-  return MPPIB_OK;
+  return e->timer.read(out);
 }
 
 int mppib_get_launch_info(mppib_engine* e, int* grid, int* block, int* smem_bytes, int* uses_tma,

@@ -10,10 +10,12 @@
  * revision (kEngineAbi is checked at registration).
  * An engine keeps a pointer to its pair's entry and one K1Plan: the form and geometry of its rollout kernel, chosen once
  * by engine.cu's choose_k1. Pair<>::kernel maps the plan's form to the instantiation that launches.
- * Three parts of the engine have an owner of their own, declared in their headers and defined in engine.cu: the noise
+ * Four parts of the engine have an owner of their own, declared in their headers and defined in engine.cu: the noise
  * draw (NoiseSource, noise_source.cuh), the merge from K1's block partials to the result record (Reduction,
- * reduction.cuh) and the model's blobs: parameters, weights and maps (ModelParams, model_params.cuh). K1 reads the
- * current noise buffer, writes the partials and takes the model's blobs through their accessors.
+ * reduction.cuh), the model's blobs: parameters, weights and maps (ModelParams, model_params.cuh), and the feedback
+ * controller: DDP's weights and workspace and RMPPI's gains (Feedback, feedback.cuh). K1 reads the current noise buffer,
+ * writes the partials and takes the model's blobs and the gains through their accessors; the DDP launch reads the
+ * weights. The stage timing of a solve is a fifth, StageTimer, declared below.
  */
 #pragma once
 #include <cuda.h>
@@ -34,6 +36,7 @@
 #include "combine_kernel.cuh"
 #include "ddp_kernel.cuh"
 #include "device_resources.cuh"
+#include "feedback.cuh"
 #include "model_params.cuh"
 #include "noise_source.cuh"
 #include "plugins/costs.cuh"
@@ -100,6 +103,29 @@ struct K1Plan
 
 struct PairEntry;
 
+// ---- stage timing (mppib_enable_timing / mppib_get_timing; definitions in engine.cu) -----------------------------------
+// Events at the start of a solve, after the noise draw, after K1 and after K2. Whether a solve is timed is decided once, as
+// it is enqueued; a drained solve adds a sample only if it was timed and timing is still on. With several solves in flight
+// the events hold the last one's, which alone is counted.
+class StageTimer : NoCopy
+{
+public:
+  cudaError_t create();
+  void enable(bool on);  // and reset the sums
+  // a solve is being enqueued: it is timed iff timing is on; stage 0, then stages i = 1 .. 3
+  cudaError_t start(cudaStream_t s) { timed_ = on_; return mark(0, s); }
+  cudaError_t mark(int i, cudaStream_t s) { return timed_ ? cudaEventRecord(ev_[i], s) : cudaSuccess; }
+  bool timed() const { return timed_; }  // the solve enqueued last
+  void collect();                        // after the stream has drained: one sample, if that solve counts
+  int read(mppib_timing* out) const;
+
+private:
+  Event ev_[4];
+  bool on_ = false, timed_ = false;
+  double sum_ms_[4] = { 0, 0, 0, 0 };
+  long n_ = 0;
+};
+
 // ---- engine state -----------------------------------------------------------------------------------------------
 // Every device resource is a member that releases itself (device_resources.cuh); a buffer that grows does so through
 // reserve(). ~mppib_engine (engine.cu) drains the stream and releases what must go before it; the members follow.
@@ -121,9 +147,7 @@ struct mppib_engine
   int num_sms = 0;  // multiprocessors of the device (grid-stride kernels launch up to 16 CTAs per SM)
   bool writeback = false;
   bool rmppi = false;  // MPPIB_FLAG_RMPPI
-  float value_func_threshold = 1000.0f;  // robust_mppi_controller.cuh default
-  DeviceBuffer<float> fb_gains_d;        // [T][S][C] or null
-  DeviceBuffer<float> eval_states_d;     // init-eval scratch: candidates, strides, costs
+  DeviceBuffer<float> eval_states_d;  // init-eval scratch: candidates, strides, costs
   DeviceBuffer<int> eval_strides_d;
   DeviceBuffer<float> eval_costs_d;
   // sampled (visualisation) trajectories scratch: picked indices, optimised sequence, outputs / costs / crash flags
@@ -135,18 +159,13 @@ struct mppib_engine
   DeviceBuffer<float> vis_outputs_d;
   DeviceBuffer<float> vis_costs_d;
   DeviceBuffer<int> vis_crash_d;
-  // DDP feedback (ddp_kernel.cuh, mppib_set_ddp / mppib_ddp_feedback): weights (empty = identity, DDPParams defaults), the
-  // workspace for the longest horizon so far and the solve's status word
-  std::vector<float> ddp_Q, ddp_Qf, ddp_R;
-  int ddp_iters = 1;
-  DeviceBuffer<float> ddp_ws_d;
-  DeviceBuffer<int> ddp_status_d;
 
   // solver scalars
   float dt = 0.01f, lambda = 1.0f, alpha = 0.0f;
 
   ModelParams model;  // the dynamics and cost blobs, weights and maps (model_params.cuh)
   NoiseSource noise;  // K0 / K0c / NLN draw, its sampler parameters, two buffers and prefetch (noise_source.cuh)
+  Feedback feedback;  // DDP's weights, workspace and status, RMPPI's gains and value-function threshold (feedback.cuh)
 
   // device buffers
   DeviceBuffer<float> costs_d;        // [D][n_local]
@@ -154,19 +173,12 @@ struct mppib_engine
   DeviceBuffer<float> weights_d;      // lazily allocated for mppib_get_weights
   DeviceBuffer<unsigned char> l2_flush_d;  // optional: all of it is written between K0 and K1 to evict the noise from L2
   int pending = 0;               // solves enqueued and not yet waited for
-  // accumulated stage timings (timing mode)
-  double acc_ms[4] = { 0, 0, 0, 0 };
-  long acc_n = 0;
 
   CUtensorMap tmap[2]{};  // K1's TMA view of noise.buffer(i) (its box is K1's block width)
 
   // K1's block partials, K2 and the cross-rank merge, the result record, Tsallis weights, NCCL and KX (reduction.cuh)
   Reduction reduction;
-
-  // timing
-  bool timing = false;
-  Event ev[4];
-  bool timing_valid = false;
+  StageTimer timer;
 
   bool solved_once = false;
 };
@@ -341,8 +353,8 @@ struct Pair
     a.dyn_shared_floats = e.k1.dyn_shared_floats;
     a.ring = e.k1.stream ? e.k1.ring : 0;
     a.stream_readback = e.k1.stream_readback ? 1 : 0;
-    a.fb_gains = e.fb_gains_d;
-    a.value_func_threshold = e.value_func_threshold;
+    a.fb_gains = e.feedback.gains();
+    a.value_func_threshold = e.feedback.threshold();
     a.lambda_inv = (float)(1.0 / e.lambda);  // mppi_controller.cu:201-202: 1.0 / lambda in double, narrowed
     memcpy(a.x0, x0, sizeof(float) * e.D * e.S);
     memcpy(a.means, U_in, sizeof(float) * e.D * e.TC);
@@ -433,23 +445,20 @@ static int nominal_traj_launch(mppib_engine& e, const float* x0, const float* u_
   return launch_helper_kernel<DYN>(nominal_traj_kernel<DYN>, a, e, 0, 1);
 }
 
-// DDPFeedback::computeFeedback for this pair's dynamics (ddp_kernel.cuh): the workspace already holds the targets and the
-// initial controls; gains_d = the destination of the gain trajectory, or null
+// DDPFeedback::computeFeedback for this pair's dynamics (ddp_kernel.cuh), with e.feedback's weights, workspace and status
+// word (Feedback::compute has put the targets and the initial controls in the workspace); gains_d = the destination of
+// the gain trajectory, or null
 template <class DYN>
 static int ddp_launch(mppib_engine& e, int T, const float* x0, float* gains_d)
 {
   using Args = ddp::DdpArgs<DYN>;
-  constexpr int S = DYN::STATE_DIM, C = DYN::CONTROL_DIM;
+  constexpr int C = DYN::CONTROL_DIM;
   static_assert(sizeof(Args) < 4000, "kernel parameter block too large");
   Args a;
   fill_dyn_args(a.dyn, a.aux, e);
-  for (int i = 0; i < S * S; i++)
-  {
-    a.Q[i] = e.ddp_Q.empty() ? (i % (S + 1) == 0 ? 1.0f : 0.0f) : e.ddp_Q[i];
-    a.Qf[i] = e.ddp_Qf.empty() ? (i % (S + 1) == 0 ? 1.0f : 0.0f) : e.ddp_Qf[i];
-  }
-  for (int i = 0; i < C * C; i++)
-    a.R[i] = e.ddp_R.empty() ? (i % (C + 1) == 0 ? 1.0f : 0.0f) : e.ddp_R[i];
+  memcpy(a.Q, e.feedback.Q(), sizeof(a.Q));
+  memcpy(a.Qf, e.feedback.Q_f(), sizeof(a.Qf));
+  memcpy(a.R, e.feedback.R(), sizeof(a.R));
   memcpy(a.x0, x0, sizeof(a.x0));
   for (int c = 0; c < C; c++)
   {
@@ -458,10 +467,10 @@ static int ddp_launch(mppib_engine& e, int T, const float* x0, float* gains_d)
   }
   a.dt = e.dt;
   a.T = T;
-  a.iters = e.ddp_iters;
-  a.ws = e.ddp_ws_d;
+  a.iters = e.feedback.iters();
+  a.ws = e.feedback.ws();
   a.gains = gains_d;
-  a.status = e.ddp_status_d;
+  a.status = e.feedback.status();
   ddp::ddp_kernel<DYN><<<1, ddp::kThreads, 0, e.stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   return MPPIB_OK;

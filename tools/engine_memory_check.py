@@ -1,7 +1,8 @@
 """Check that an engine gives back every byte of device memory it took, after each buffer that grows or is freed on
 demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
   - an RMPPI engine (quadrotor + QuadrotorMapCost, D = 2): solve, init-eval twice with more candidates the second time, the
-    cost map replaced by one with four times the cells, the feedback gains set, freed and set again, a solve after each;
+    cost map replaced by one with four times the cells, a DDP at the horizon that writes the feedback gains, a longer DDP
+    that grows its workspace, the feedback gains freed and set again, a solve after each;
   - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time;
   - a ColoredNoise and an NLN engine (the samplers whose spectrum, plan and log-normal planes the noise source owns): solve,
     new sampler parameters, solve, burn_draws, solve;
@@ -45,6 +46,9 @@ def exercise():
     w.cost.tex_helper_ = W.quadrotor_track_map(resolution=0.125)[0]
     e.push_cost()
     e.solve(x0, U)
+    for T, to_rmppi in ((w.T, True), (3 * w.T, False)):  # hover targets; the second horizon grows the DDP workspace
+        e.ddp_feedback(x0[0], np.tile(x0[0], (T, 1)), np.tile(U[0, :1], (T, 1)), to_rmppi=to_rmppi)
+        e.solve(x0, U)
     e.set_rmppi(3000.0, None)
     e.solve(x0, U)
     e.set_rmppi(3000.0, gains)
