@@ -193,10 +193,10 @@ private:
   mppib_engine* engineForSolve()
   {
     if (!engine_)
-    {  // standalone: one small engine of the model's in-tree pair (dynamics id == cost id for every pair with a Jacobian)
+    {  // standalone: one small engine of the model's in-tree pair (Dynamics::DDP_COST_ID)
       mppib_desc d{};
       d.dynamics_id = DYN_T::DYN_ID;
-      d.cost_id = DYN_T::DYN_ID;
+      d.cost_id = DYN_T::DDP_COST_ID;
       d.num_rollouts = 32;
       d.num_timesteps = 2;
       d.num_distributions = 1;

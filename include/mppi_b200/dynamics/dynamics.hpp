@@ -23,6 +23,9 @@ public:
   static const int CONTROL_DIM = C_DIM;
   static const int OUTPUT_DIM = O_DIM;
   static const int DYN_ID = DYN_ID_V;
+  // the cost of the small engine a standalone DDPFeedback solves on (ddp.cuh): the id of the model's in-tree pair, equal to
+  // the dynamics id for every model with a Jacobian but RacerDubinsElevation, which shadows it
+  static const int DDP_COST_ID = DYN_ID_V;
   typedef BLOB_T BLOB;
   typedef Eigen::Matrix<float, C_DIM, 1> control_array;
   typedef Eigen::Matrix<float, S_DIM, 1> state_array;

@@ -50,6 +50,16 @@ int mppib_host_step_lstm(const void* dyn_params, const mppib_host_lstm* net, con
                          float* x_next, float* xdot, float* y);
 int mppib_host_output_trajectory_lstm(const void* dyn_params, const mppib_host_lstm* net, const float* x0,
                                       const float* u, int T, float dt, float* states, float* outputs);
+/* RacerDubinsElevation (racer_dubins_elevation.cu:229-255, host step): the host body, which differs from the device one
+ * (DESIGN §8) in sinf / tanf / sincosf without normalizeAngle and in its brake clamp [0, -control_rngs_[0].x]. map may be
+ * NULL (flat ground). */
+int mppib_host_step_racer_dubins_elevation(const void* dyn_params, const mppib_elevation_map_header* map, const float* x,
+                                           const float* u, float dt, float* x_next, float* xdot, float* y);
+/* RacerDubinsElevation::computeGrad (racer_dubins_elevation.cu:257-334): A [19][19] and B [19][2], row-major. */
+int mppib_host_grad_racer_dubins_elevation(const void* dyn_params, const float* x, const float* u, float* A, float* B);
+int mppib_host_output_trajectory_racer_dubins_elevation(const void* dyn_params, const mppib_elevation_map_header* map,
+                                                        const float* x0, const float* u, int T, float dt, float* states,
+                                                        float* outputs);
 /* LSTMLSTMHelper::initializeLSTM (utils/nn_helpers/lstm_lstm_helper.cu:50-73): the INIT network — an LSTM (input_dim, hidden_dim)
  * with an FNN head on [h; x] (layers {hidden_dim + input_dim, ..., 2 * H_prediction}) — runs over the last init_len columns
  * of a buffer of past inputs, starting from its own initial hidden / cell state; the head's output after the last column is

@@ -25,6 +25,7 @@ enum mppib_dynamics_id
   MPPIB_DYN_AUTORALLY_NN = 2,      /* dynamics/autorally/ar_nn_model.cuh NeuralNetModel<7,2,3>  S7 C2 O8 */
   MPPIB_DYN_RACER_LSTM = 3,        /* dynamics/racer_dubins/racer_dubins_elevation_lstm_steering.cuh S19 C2 O28 */
   MPPIB_DYN_QUADROTOR = 4,         /* dynamics/quadrotor/quadrotor_dynamics.cuh          S13 C4 O13 */
+  MPPIB_DYN_RACER_DUBINS_ELEVATION = 5, /* dynamics/racer_dubins/racer_dubins_elevation.cuh  S19 C2 O28 */
   MPPIB_DYN_COUNT
 };
 
@@ -124,6 +125,11 @@ typedef struct mppib_racer_lstm_dyn_params
   float Q_omega_v;                 /* 0.001 */
   float Q_omega_steering;          /* 0 */
 } mppib_racer_lstm_dyn_params;
+
+/* RacerDubinsElevation (dynamics/racer_dubins/racer_dubins_elevation.cuh): RacerDubinsElevationParams, the same fields as
+ * the LSTM model's blob, which carries exactly them. steer_accel_constant / steer_accel_drag_constant are unused by this
+ * model (its steering is first order, racer_dubins.cu:296-304). Map: MPPIB_BLOB_ELEVATION_MAP; no weights. */
+typedef mppib_racer_lstm_dyn_params mppib_racer_dubins_elevation_dyn_params;
 
 /* Elevation map of the RACER models (utils/texture_helpers/texture_helper.cuh:11-56 TextureParams + two_d_texture_helper.cu):
  * MPPIB_BLOB_ELEVATION_MAP = this header followed by width * height floats, row-major (value at row i, column j =

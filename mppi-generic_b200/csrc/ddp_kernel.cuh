@@ -36,7 +36,7 @@ namespace mppib
 namespace ddp
 {
 constexpr int kThreads = 256;
-constexpr int kMaxS = 16, kMaxC = 4;
+constexpr int kMaxS = 20, kMaxC = 4;
 
 // offsets (floats) of the workspace arrays for horizon T
 struct WsLayout
@@ -172,7 +172,7 @@ template <class DYN>
 __global__ void __launch_bounds__(kThreads, 1) ddp_kernel(const __grid_constant__ DdpArgs<DYN> a)
 {
   constexpr int S = DYN::STATE_DIM, C = DYN::CONTROL_DIM, SC = S + C;
-  static_assert(S <= kMaxS && C <= kMaxC, "DDP is built for STATE_DIM <= 16, CONTROL_DIM <= 4");
+  static_assert(S <= kMaxS && C <= kMaxC, "DDP is built for STATE_DIM <= 20, CONTROL_DIM <= 4");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, T = a.T;
   const float dt = a.dt;
   const WsLayout L = ws_layout(T, S, C);

@@ -110,6 +110,8 @@ static const PairEntry kPairs[] = {
   make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorQuadraticCost>(MPPIB_DYN_QUADROTOR,
                                                                           MPPIB_COST_QUADROTOR_QUADRATIC),
   make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorMapCost>(MPPIB_DYN_QUADROTOR, MPPIB_COST_QUADROTOR_MAP),
+  make_entry<plugins::RacerDubinsElevationDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_DUBINS_ELEVATION,
+                                                                                 MPPIB_COST_RACER_QUADRATIC),
 };
 
 // RacerDubinsElevationLSTMSteering with the steering LSTM on tensor cores (hidden_dim 32, head width <= 24)
@@ -1241,8 +1243,9 @@ bool ModelParams::uses(int which) const
     case MPPIB_BLOB_NN_WEIGHTS:
       return dyn_id_ == MPPIB_DYN_AUTORALLY_NN;
     case MPPIB_BLOB_LSTM_WEIGHTS:
-    case MPPIB_BLOB_ELEVATION_MAP:
       return dyn_id_ == MPPIB_DYN_RACER_LSTM;
+    case MPPIB_BLOB_ELEVATION_MAP:
+      return dyn_id_ == MPPIB_DYN_RACER_LSTM || dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION;
     case MPPIB_BLOB_COSTMAP:  // the costs whose blobs share the mppib_ar_standard_cost_params prefix
       return cost_id_ == MPPIB_COST_AR_STANDARD || cost_id_ == MPPIB_COST_AR_ROBUST;
     case MPPIB_BLOB_COST_TEXTURE:
@@ -1419,6 +1422,10 @@ int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, flo
                                is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr };
     return mppib_host_output_trajectory_lstm(dyn_.data(), &net, x0, u, T, dt, states, outputs);
   }
+  if (dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION)
+    return mppib_host_output_trajectory_racer_dubins_elevation(
+        dyn_.data(), is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr, x0, u,
+        T, dt, states, outputs);
   return mppib_host_output_trajectory(dyn_id_, dyn_.data(), is_set(MPPIB_BLOB_NN_WEIGHTS) ? nn_.h.data() : nullptr, x0, u,
                                       T, dt, states, outputs);
 }

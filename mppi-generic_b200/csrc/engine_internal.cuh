@@ -211,6 +211,14 @@ struct AuxFill<plugins::RacerLSTMDynamics::Aux>
   }
 };
 template <>
+struct AuxFill<plugins::RacerDubinsElevationDynamics::Aux>
+{
+  static void fill(plugins::RacerDubinsElevationDynamics::Aux& a, const ModelParams& m)
+  {
+    a.elev = m.elevation_map();
+  }
+};
+template <>
 struct AuxFill<plugins::ARStandardCost::Aux>
 {
   static void fill(plugins::ARStandardCost::Aux& a, const ModelParams& m)

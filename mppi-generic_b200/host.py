@@ -28,6 +28,7 @@ FLT_MAX = 3.4028234663852886e38
 
 # plugin ids (include/mppi_b200/params.h)
 DYN_CARTPOLE, DYN_DOUBLE_INTEGRATOR, DYN_AUTORALLY_NN, DYN_RACER_LSTM, DYN_QUADROTOR = 0, 1, 2, 3, 4
+DYN_RACER_DUBINS_ELEVATION = 5
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
 COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
 COST_QUADROTOR_MAP = 7
@@ -317,6 +318,8 @@ ABI_SYMBOLS = [
     "mppib_host_dims", "mppib_host_enforce_constraints", "mppib_host_step", "mppib_host_smooth_controls",
     "mppib_host_slide_controls", "mppib_host_output_trajectory", "mppib_host_free_energy",
     "mppib_host_merge_records", "mppib_host_step_lstm", "mppib_host_output_trajectory_lstm",
+    "mppib_host_step_racer_dubins_elevation", "mppib_host_output_trajectory_racer_dubins_elevation",
+    "mppib_host_grad_racer_dubins_elevation",
     "mppib_host_elevation_at_world_pose", "mppib_host_static_settling", "mppib_host_lstm_initialize",
     "mppib_set_rmppi", "mppib_init_eval", "mppib_set_tsallis", "mppib_sample_trajectories", "mppib_nominal_trajectory", "mppib_compute_control", "mppib_host_npz_read", "mppib_comm_p2p_handle", "mppib_comm_p2p_open", "mppib_host_rmppi_line_search_weights", "mppib_host_rmppi_candidates",
     "mppib_host_rmppi_best_index", "mppib_set_ddp", "mppib_ddp_feedback",
@@ -385,6 +388,9 @@ def lib() -> C.CDLL:
     L.mppib_host_output_trajectory.argtypes = [C.c_int, vp, vp, vp, vp, C.c_int, C.c_float, vp, vp]
     L.mppib_host_step_lstm.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, C.c_float, vp, vp, vp]
     L.mppib_host_output_trajectory_lstm.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, C.c_int, C.c_float, vp, vp]
+    L.mppib_host_step_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, C.c_float, vp, vp, vp]
+    L.mppib_host_output_trajectory_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, C.c_int, C.c_float, vp, vp]
+    L.mppib_host_grad_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, vp]
     L.mppib_set_rmppi.argtypes = [vp, C.c_float, vp]
     L.mppib_set_tsallis.argtypes = [vp, C.c_float, C.c_float]
     L.mppib_init_eval.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]
@@ -587,15 +593,12 @@ def npz_read(path: str, name: str) -> np.ndarray:
     return out.reshape([shape[i] for i in range(ndim.value)])
 
 
-class RacerDubinsElevationLSTMSteering(_Dynamics):
-    """dynamics/racer_dubins/racer_dubins_elevation_lstm_steering.cuh:34-49 —
-    RacerDubinsElevationLSTMSteering(init_input_dim, init_hidden_dim, init_output_layers, input_dim, hidden_dim,
-    output_layers, init_len). The prediction LSTM (input_dim must be 4, output_layers = [hidden_dim + 4, L1, 1]) runs
-    inside the rollout; the init network (LSTMLSTMHelper) only produces the initial hidden / cell state from a history
-    buffer on the host (updateFromBuffer, :215-232) and is represented here by that state itself
-    (``setInitialHiddenCell``), or computed by the init network itself (``setAllValuesInit`` / ``loadParamsInit`` +
-    ``initializeLSTM`` / ``updateFromBuffer``). Elevation map: ``getTextureHelper()`` / ``setElevationMap``."""
-    DYN_ID, STATE_DIM, CONTROL_DIM, OUTPUT_DIM = DYN_RACER_LSTM, 19, 2, 28
+class RacerDubinsElevation(_Dynamics):
+    """dynamics/racer_dubins/racer_dubins_elevation.cuh — RacerDubinsElevation() / RacerDubinsElevation(params): the
+    parametric RACER vehicle (S19 C2 O28) with first-order steering and no per-sample memory, so Tube-MPPI and RMPPI roll it
+    out. Its blob is RacerDubinsElevationParams (params.h: mppib_racer_dubins_elevation_dyn_params). Elevation map:
+    ``getTextureHelper()`` / ``setElevationMap``."""
+    DYN_ID, STATE_DIM, CONTROL_DIM, OUTPUT_DIM = DYN_RACER_DUBINS_ELEVATION, 19, 2, 28
 
     def enforceLeash(self, state_true, state_nominal, leash_values) -> np.ndarray:
         """RacerDubinsImpl::enforceLeash (racer_dubins.cu:177-230): x / y leashed in the body frame of the true state, yaw by
@@ -626,27 +629,8 @@ class RacerDubinsElevationLSTMSteering(_Dynamics):
                 out[i] = n[i]
         return out.astype(np.float32)
 
-    def __init__(self, init_input_dim: int = 3, init_hidden_dim: int = 20, init_output_layers: Sequence[int] = (23, 100, 8),
-                 input_dim: int = 4, hidden_dim: int = 4, output_layers: Sequence[int] = (8, 20, 1), init_len: int = 11):
+    def __init__(self, params: Optional[RacerLSTMDynParams] = None):
         super().__init__()
-        output_layers = tuple(output_layers)
-        if input_dim != RACER_LSTM_INPUT_DIM:
-            raise ValueError("the steering LSTM takes 4 inputs (lstm_steering.cu:148-151)")
-        if len(output_layers) != 3 or output_layers[0] != hidden_dim + input_dim or output_layers[2] != 1:
-            raise ValueError("output_layers must be [hidden_dim + 4, L1, 1] (lstm_helper.cu:41)")
-        if tuple(init_output_layers)[-1] != 2 * hidden_dim:
-            raise ValueError("init network must output 2 * hidden_dim values (lstm_lstm_helper.cu:11)")
-        self.hidden_dim, self.head_hidden = hidden_dim, output_layers[1]
-        # the init network (LSTMLSTMHelper::init_model_, lstm_lstm_helper.cu:4-12): host-only, zero-initialised like the
-        # reference's constructor leaves it
-        self.init_input_dim, self.init_hidden_dim, self.init_len = init_input_dim, init_hidden_dim, init_len
-        self.init_output_layers = tuple(int(v) for v in init_output_layers)
-        if self.init_output_layers[0] != init_hidden_dim + init_input_dim:
-            raise ValueError("init_output_layers[0] must be init_hidden_dim + init_input_dim (lstm_helper.cu:41)")
-        Hi, Ii = init_hidden_dim, init_input_dim
-        self.init_lstm_theta = np.zeros(4 * Hi * Hi + 4 * Hi * Ii + 6 * Hi, np.float32)
-        self.init_head_theta = np.zeros(sum(a * b + b for a, b in zip(self.init_output_layers[:-1],
-                                                                     self.init_output_layers[1:])), np.float32)
         p = RacerLSTMDynParams()
         p.lim.set_defaults()
         # racer_dubins.cuh:78-104, racer_dubins_elevation.cuh:47-59
@@ -670,8 +654,17 @@ class RacerDubinsElevationLSTMSteering(_Dynamics):
             p.Q_x_v[i] = v
         p.Q_y_f, p.Q_omega_v, p.Q_omega_steering = 0.1, 0.001, 0.0
         self.params = p
-        self.lstm_theta = np.zeros(racer_lstm_num_params(self.hidden_dim, self.head_hidden), np.float32)
+        if params is not None:
+            C.memmove(C.byref(self.params), C.byref(params), C.sizeof(RacerLSTMDynParams))
         self.tex_helper_ = TwoDTextureHelper()  # racer_dubins_elevation.cuh: tex_helper_ (map 0 = elevation)
+
+    def getParams(self) -> RacerLSTMDynParams:
+        out = RacerLSTMDynParams()
+        C.memmove(C.byref(out), C.byref(self.params), C.sizeof(RacerLSTMDynParams))
+        return out
+
+    def setParams(self, params: RacerLSTMDynParams) -> None:
+        C.memmove(C.byref(self.params), C.byref(params), C.sizeof(RacerLSTMDynParams))
 
     def getTextureHelper(self) -> "TwoDTextureHelper":
         return self.tex_helper_
@@ -698,6 +691,64 @@ class RacerDubinsElevationLSTMSteering(_Dynamics):
         r, p_ = C.c_float(roll), C.c_float(pitch)
         h = L.mppib_host_static_settling(None if b is None else b.ctypes.data, yaw, x, y, C.byref(r), C.byref(p_))
         return r.value, p_.value, float(h)
+
+    def _map_ptr(self):
+        b = self.tex_helper_.blob()
+        return None if b is None else b.ctypes.data
+
+    def step(self, state, control, dt: float):
+        """Host step (racer_dubins_elevation.cu:229-255); returns (next_state, state_der, output)."""
+        x, u = _f32(state), _f32(control)
+        xn, xd, y = np.zeros(19, np.float32), np.zeros(19, np.float32), np.zeros(28, np.float32)
+        _check(lib().mppib_host_step_racer_dubins_elevation(C.addressof(self.params), self._map_ptr(), _ptr(x), _ptr(u),
+                                                             dt, _ptr(xn), _ptr(xd), _ptr(y)))
+        return xn, xd, y
+
+    def computeGrad(self, state, control):
+        """RacerDubinsElevationImpl::computeGrad (racer_dubins_elevation.cu:257-334): returns (A [19][19], B [19][2])."""
+        A, B = np.zeros((19, 19), np.float32), np.zeros((19, 2), np.float32)
+        _check(lib().mppib_host_grad_racer_dubins_elevation(C.addressof(self.params), _ptr(_f32(state)), _ptr(_f32(control)),
+                                                             _ptr(A), _ptr(B)))
+        return A, B
+
+    def output_trajectory(self, x0, u, T: int, dt: float, states: np.ndarray, outputs: np.ndarray) -> None:
+        _check(lib().mppib_host_output_trajectory_racer_dubins_elevation(C.addressof(self.params), self._map_ptr(),
+                                                                          _ptr(_f32(x0)), _ptr(_f32(u)), T, dt,
+                                                                          _ptr(states), _ptr(outputs)))
+
+
+class RacerDubinsElevationLSTMSteering(RacerDubinsElevation):
+    """dynamics/racer_dubins/racer_dubins_elevation_lstm_steering.cuh:34-49 —
+    RacerDubinsElevationLSTMSteering(init_input_dim, init_hidden_dim, init_output_layers, input_dim, hidden_dim,
+    output_layers, init_len). The prediction LSTM (input_dim must be 4, output_layers = [hidden_dim + 4, L1, 1]) runs
+    inside the rollout; the init network (LSTMLSTMHelper) only produces the initial hidden / cell state from a history
+    buffer on the host (updateFromBuffer, :215-232) and is represented here by that state itself
+    (``setInitialHiddenCell``), or computed by the init network itself (``setAllValuesInit`` / ``loadParamsInit`` +
+    ``initializeLSTM`` / ``updateFromBuffer``). Elevation map: ``getTextureHelper()`` / ``setElevationMap``."""
+    DYN_ID, STATE_DIM, CONTROL_DIM, OUTPUT_DIM = DYN_RACER_LSTM, 19, 2, 28
+
+    def __init__(self, init_input_dim: int = 3, init_hidden_dim: int = 20, init_output_layers: Sequence[int] = (23, 100, 8),
+                 input_dim: int = 4, hidden_dim: int = 4, output_layers: Sequence[int] = (8, 20, 1), init_len: int = 11):
+        super().__init__()
+        output_layers = tuple(output_layers)
+        if input_dim != RACER_LSTM_INPUT_DIM:
+            raise ValueError("the steering LSTM takes 4 inputs (lstm_steering.cu:148-151)")
+        if len(output_layers) != 3 or output_layers[0] != hidden_dim + input_dim or output_layers[2] != 1:
+            raise ValueError("output_layers must be [hidden_dim + 4, L1, 1] (lstm_helper.cu:41)")
+        if tuple(init_output_layers)[-1] != 2 * hidden_dim:
+            raise ValueError("init network must output 2 * hidden_dim values (lstm_lstm_helper.cu:11)")
+        self.hidden_dim, self.head_hidden = hidden_dim, output_layers[1]
+        # the init network (LSTMLSTMHelper::init_model_, lstm_lstm_helper.cu:4-12): host-only, zero-initialised like the
+        # reference's constructor leaves it
+        self.init_input_dim, self.init_hidden_dim, self.init_len = init_input_dim, init_hidden_dim, init_len
+        self.init_output_layers = tuple(int(v) for v in init_output_layers)
+        if self.init_output_layers[0] != init_hidden_dim + init_input_dim:
+            raise ValueError("init_output_layers[0] must be init_hidden_dim + init_input_dim (lstm_helper.cu:41)")
+        Hi, Ii = init_hidden_dim, init_input_dim
+        self.init_lstm_theta = np.zeros(4 * Hi * Hi + 4 * Hi * Ii + 6 * Hi, np.float32)
+        self.init_head_theta = np.zeros(sum(a * b + b for a, b in zip(self.init_output_layers[:-1],
+                                                                     self.init_output_layers[1:])), np.float32)
+        self.lstm_theta = np.zeros(racer_lstm_num_params(self.hidden_dim, self.head_hidden), np.float32)
 
     def model_dims(self) -> Sequence[int]:
         return (self.hidden_dim, self.head_hidden)
@@ -1316,6 +1367,7 @@ class Engine:
         if self.dyn.DYN_ID == DYN_RACER_LSTM:
             w = _f32(self.dyn.lstm_theta)
             _check(L.mppib_set_blob(self._h, BLOB_LSTM_WEIGHTS, _ptr(w), w.nbytes))
+        if self.dyn.DYN_ID in (DYN_RACER_LSTM, DYN_RACER_DUBINS_ELEVATION):
             m = self.dyn.tex_helper_.blob()
             if m is not None:  # TwoDTextureHelper::copyToDevice
                 _check(L.mppib_set_blob(self._h, BLOB_ELEVATION_MAP, m.ctypes.data, m.nbytes))

@@ -214,6 +214,52 @@ def racer_lstm_h32(N: int = 65536, T: int = 150) -> Workload:
     return racer_lstm(N, T, hidden_dim=32, head_hidden=20)
 
 
+def racer_elevation_map(seed: int = 11, resolution: float = 0.5) -> "H.TwoDTextureHelper":
+    """A rolling elevation map for the RACER workloads: x in [-10, 90], y in [-30, 30] m, heights from two gentle sine waves
+    (amplitude 0.4 and 0.25 m, wavelengths 24 and 15 m) plus seeded noise in [0, 0.02) m."""
+    xb, yb = (-10.0, 90.0), (-30.0, 30.0)
+    w, h = int(round((xb[1] - xb[0]) / resolution)), int(round((yb[1] - yb[0]) / resolution))
+    cx = xb[0] + (np.arange(w) + 0.5) * resolution
+    cy = yb[0] + (np.arange(h) + 0.5) * resolution
+    X, Y = np.meshgrid(cx, cy)  # [h][w]
+    z = 0.4 * np.sin(2 * math.pi * X / 24.0) + 0.25 * np.cos(2 * math.pi * Y / 15.0)
+    z = (z + 0.02 * np.random.RandomState(seed).uniform(0.0, 1.0, z.shape)).astype(np.float32)
+    tex = H.TwoDTextureHelper()
+    tex.setExtent(0, w, h)
+    tex.updateTexture(0, z)
+    tex.updateOrigin(0, (xb[0], yb[0], 0.0))
+    tex.updateResolution(0, resolution)
+    tex.enableTexture(0)
+    return tex
+
+
+def racer_elevation(N: int = 8192, T: int = 100, use_map: bool = True) -> Workload:
+    """RacerDubinsElevation (reference default parameters) + our quadratic tracking cost, VanillaMPPI: hold 1.2 m/s along
+    +x over racer_elevation_map() (flat ground when use_map is False)."""
+    dyn = H.RacerDubinsElevation()
+    dyn.setControlRanges([(-1.0, 1.0), (-1.0, 1.0)])  # throttle/brake, steering command
+    if use_map:
+        dyn.tex_helper_ = racer_elevation_map()
+    cost = H.RacerQuadraticCost()
+    cost.params.desired_speed = 1.2
+    sampler = H.GaussianDistribution(2, [0.3, 0.3])
+    x0 = np.zeros((1, 19), np.float32)
+    x0[0, 0] = 1.0  # VEL_X
+    x0[0, 9:13] = 1e-6  # covariance diagonal floor
+    U0 = np.zeros((1, T, 2), np.float32)
+    return Workload(f"racer_elevation{'' if use_map else '_nomap'}_N{N}_T{T}", "vanilla", dyn, cost, sampler, N, T, 1, 0.02,
+                    1.0, 0.0, x0, U0)
+
+
+def racer_elevation_tube(N: int = 8192, T: int = 100, use_map: bool = True) -> Workload:
+    """racer_elevation() with Tube-MPPI: two distributions, the nominal and the real system."""
+    w = racer_elevation(N, T, use_map)
+    w.name, w.controller, w.D = f"racer_elevation_tube{'' if use_map else '_nomap'}_N{N}_T{T}", "tube", 2
+    w.x0, w.U0 = np.tile(w.x0, (2, 1)), np.tile(w.U0, (2, 1, 1))
+    w.extra = {"nominal_threshold": 20.0}
+    return w
+
+
 def quadrotor(N: int = 8192, T: int = 100) -> Workload:
     """Quadrotor + quadratic cost, VanillaMPPI (instantiations/quadrotor_mppi/quadrotor_mppi.cuh): fly from the origin
     to a goal 4 m away and 2 m up, hovering there. The only CONTROL_DIM = 4 pair (one 16-byte noise group per step)."""
@@ -315,6 +361,8 @@ BUILDERS = {
     "double_integrator_robust_tube": double_integrator_robust_tube,
     "quadrotor": quadrotor,
     "quadrotor_gates": quadrotor_gates,
+    "racer_elevation": racer_elevation,
+    "racer_elevation_tube": racer_elevation_tube,
 }
 
 
