@@ -74,7 +74,7 @@ private:
   size_t n_ = 0;
 };
 
-// Pinned host memory (cudaHostAlloc), allocated once.
+// Pinned host memory (cudaHostAlloc): pointer + capacity in elements.
 template <class T>
 class PinnedBuffer : NoCopy
 {
@@ -88,17 +88,35 @@ public:
   {
     return p_;
   }
-  // n elements with the cudaHostAlloc* flags given; for cudaHostAllocMapped memory, *device_alias = the address kernels use
+  // n elements with the cudaHostAlloc* flags given, allocated once; for cudaHostAllocMapped memory, *device_alias = the
+  // address kernels use
   cudaError_t alloc(size_t n, unsigned flags, T** device_alias = nullptr)
   {
     cudaError_t rc = cudaHostAlloc((void**)&p_, n * sizeof(T), flags);
+    if (rc == cudaSuccess)
+      n_ = n;
     if (rc == cudaSuccess && device_alias)
       rc = cudaHostGetDevicePointer((void**)device_alias, (void*)p_, 0);
+    return rc;
+  }
+  // Room for n elements; the contents are not kept. No copy may still be in flight to or from it. Empty on failure.
+  cudaError_t reserve(size_t n, unsigned flags)
+  {
+    if (n <= n_)
+      return cudaSuccess;
+    if (p_)
+      cudaFreeHost((void*)p_);
+    p_ = nullptr;
+    n_ = 0;
+    const cudaError_t rc = alloc(n, flags);
+    if (rc != cudaSuccess)
+      p_ = nullptr;
     return rc;
   }
 
 private:
   T* p_ = nullptr;
+  size_t n_ = 0;
 };
 
 class Event : NoCopy

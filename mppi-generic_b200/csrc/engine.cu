@@ -1895,6 +1895,78 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
   return e->feedback.compute(*e, T, x0, x_target, u_target, to_rmppi != 0, gains, x_out, u_out, jac_out);
 }
 
+// ---- the side rollouts (side_rollouts.cuh) ----------------------------------------------------------------------------
+int SideRollouts::init_eval(mppib_engine& e, const float* candidates, const int* strides, int K, int samples,
+                            const float* U_nominal, int opt_stride, float* costs_out)
+{
+  const size_t total = (size_t)K * samples;
+  CUDA_TRY(eval_states_.reserve((size_t)K * e.S, e.stream));
+  CUDA_TRY(eval_strides_.reserve((size_t)K, e.stream));
+  CUDA_TRY(eval_costs_.reserve(total, e.stream));
+  CUDA_TRY(cudaMemcpyAsync(eval_states_, candidates, (size_t)K * e.S * sizeof(float), cudaMemcpyHostToDevice, e.stream));
+  CUDA_TRY(cudaMemcpyAsync(eval_strides_, strides, (size_t)K * sizeof(int), cudaMemcpyHostToDevice, e.stream));
+  if (int rc = e.noise.draw(opt_stride))  // sampler_->generateSamples(stride, 0, gen_) (:595)
+    return rc;
+  if (int rc = e.pair->init_eval(e, K, samples, U_nominal, opt_stride))
+    return rc;
+  CUDA_TRY(e.noise.read_by_kernel());  // the kernel above read the noise: later draws into its buffer wait for it
+  CUDA_TRY(cudaMemcpyAsync(costs_out, eval_costs_, total * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
+  CUDA_TRY(cudaStreamSynchronize(e.stream));
+  return MPPIB_OK;
+}
+
+int SideRollouts::sample(mppib_engine& e, const float* x0, const float* U_nominal, int distribution, const int* sample_idx,
+                         int n, const float* U_opt, float* outputs, float* costs, int* crash)
+{
+  const size_t n_out = (size_t)n * e.T * e.O, n_cost = (size_t)n * (e.T + 1), n_crash = (size_t)n * e.T;
+  CUDA_TRY(vis_idx_.reserve((size_t)n, e.stream));
+  CUDA_TRY(vis_outputs_.reserve(n_out, e.stream));
+  CUDA_TRY(vis_costs_.reserve(n_cost, e.stream));
+  CUDA_TRY(vis_crash_.reserve(n_crash, e.stream));
+  CUDA_TRY(cudaMemcpyAsync(vis_idx_, sample_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, e.stream));
+  have_opt_ = U_opt != nullptr;
+  if (have_opt_)
+  {
+    CUDA_TRY(vis_opt_.reserve((size_t)e.TC, e.stream));
+    CUDA_TRY(cudaMemcpyAsync(vis_opt_, U_opt, (size_t)e.TC * sizeof(float), cudaMemcpyHostToDevice, e.stream));
+  }
+  if (int rc = e.pair->sampled_traj(e, x0, U_nominal, distribution, n))
+    return rc;
+  CUDA_TRY(cudaMemcpyAsync(outputs, vis_outputs_, n_out * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
+  CUDA_TRY(cudaMemcpyAsync(costs, vis_costs_, n_cost * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
+  CUDA_TRY(cudaMemcpyAsync(crash, vis_crash_, n_crash * sizeof(int), cudaMemcpyDeviceToHost, e.stream));
+  CUDA_TRY(cudaStreamSynchronize(e.stream));
+  return MPPIB_OK;
+}
+
+int SideRollouts::nominal(mppib_engine& e, const float* x0, const float* U, const float* history, float* U_smoothed,
+                          float* states, float* outputs)
+{
+  n_u_ = (size_t)e.D * e.TC;
+  n_s_ = (size_t)e.D * e.T * e.S;
+  const size_t n = n_u_ + n_s_ + (size_t)e.D * e.T * e.O;
+  CUDA_TRY(nom_.reserve(n, e.stream));
+  CUDA_TRY(nom_h_.reserve(n, cudaHostAllocDefault));
+  nom_src_ = e.reduction.result() + kPartialHeader;  // the optimised sequence where K2 / KX left it
+  nom_stride_ = e.reduction.pstride();
+  if (U)
+  {
+    CUDA_TRY(nom_u_.reserve(n_u_, e.stream));
+    CUDA_TRY(cudaMemcpyAsync(nom_u_, U, n_u_ * sizeof(float), cudaMemcpyHostToDevice, e.stream));
+    nom_src_ = nom_u_;
+    nom_stride_ = e.TC;
+  }
+  if (int rc = e.pair->nominal_traj(e, x0, history))
+    return rc;
+  CUDA_TRY(cudaMemcpyAsync(nom_h_, nom_, n * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
+  CUDA_TRY(cudaStreamSynchronize(e.stream));
+  if (U_smoothed)
+    memcpy(U_smoothed, nom_h_, n_u_ * sizeof(float));
+  memcpy(states, nom_h_ + n_u_, n_s_ * sizeof(float));
+  memcpy(outputs, nom_h_ + n_u_ + n_s_, (n - n_u_ - n_s_) * sizeof(float));
+  return MPPIB_OK;
+}
+
 int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides, int num_candidates,
                     int samples_per_candidate, const float* U_nominal, int optimization_stride, float* costs_out)
 {
@@ -1907,26 +1979,12 @@ int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides
     return fail(MPPIB_ERR_UNSUPPORTED, "init-eval runs on one rank (a few hundred rollouts)");
   if (samples_per_candidate > e->n_local || (long)num_candidates * samples_per_candidate > e->N)
     return fail(MPPIB_ERR_INVALID_ARG, "(number of candidates) * (samples per candidate) cannot exceed NUM_ROLLOUTS");
+  for (int k = 0; k < num_candidates; k++)
+    if (strides[k] < 0)  // control min(t + stride, T - 1) of a row: a negative stride reads before the noise and the mean
+      return fail(MPPIB_ERR_INVALID_ARG, "stride %d (candidate %d) is negative", strides[k], k);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  const int total = num_candidates * samples_per_candidate;
-  CUDA_TRY(e->eval_states_d.reserve((size_t)total * e->S, e->stream));
-  CUDA_TRY(e->eval_strides_d.reserve((size_t)total, e->stream));
-  CUDA_TRY(e->eval_costs_d.reserve((size_t)total, e->stream));
-  CUDA_TRY(cudaMemcpyAsync(e->eval_states_d, candidates, (size_t)num_candidates * e->S * sizeof(float),
-                           cudaMemcpyHostToDevice, e->stream));
-  CUDA_TRY(cudaMemcpyAsync(e->eval_strides_d, strides, (size_t)num_candidates * sizeof(int), cudaMemcpyHostToDevice,
-                           e->stream));
-  rc = e->noise.draw(optimization_stride);  // sampler_->generateSamples(stride, 0, gen_) (:595)
-  if (rc != MPPIB_OK)
-    return rc;
-  rc = e->pair->init_eval(*e, e->eval_states_d, e->eval_strides_d, num_candidates, samples_per_candidate, U_nominal,
-                          optimization_stride);
-  if (rc != MPPIB_OK)
-    return rc;
-  CUDA_TRY(e->noise.read_by_kernel());  // the kernel above read the noise: later draws into its buffer wait for it
-  CUDA_TRY(cudaMemcpyAsync(costs_out, e->eval_costs_d, (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->side.init_eval(*e, candidates, strides, num_candidates, samples_per_candidate, U_nominal, optimization_stride,
+                           costs_out);
 }
 
 int mppib_sample_trajectories(mppib_engine* e, const float* x0, const float* U_nominal, int distribution,
@@ -1961,25 +2019,7 @@ int mppib_sample_trajectories(mppib_engine* e, const float* x0, const float* U_n
     if (!std::isfinite(x0[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "x0[%d] is not finite", i);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  CUDA_TRY(e->vis_idx_d.reserve((size_t)n, e->stream));
-  CUDA_TRY(e->vis_outputs_d.reserve((size_t)n * e->T * e->O, e->stream));
-  CUDA_TRY(e->vis_costs_d.reserve((size_t)n * (e->T + 1), e->stream));
-  CUDA_TRY(e->vis_crash_d.reserve((size_t)n * e->T, e->stream));
-  if (have_opt && !e->vis_opt_d)
-    CUDA_TRY(e->vis_opt_d.alloc((size_t)e->TC));
-  CUDA_TRY(cudaMemcpyAsync(e->vis_idx_d, sample_idx, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, e->stream));
-  if (have_opt)
-    CUDA_TRY(cudaMemcpyAsync(e->vis_opt_d, U_opt, (size_t)e->TC * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-  rc = e->pair->sampled_traj(*e, x0, U_nominal, distribution, n, have_opt);
-  if (rc != MPPIB_OK)
-    return rc;
-  CUDA_TRY(cudaMemcpyAsync(outputs, e->vis_outputs_d, (size_t)n * e->T * e->O * sizeof(float), cudaMemcpyDeviceToHost,
-                           e->stream));
-  CUDA_TRY(cudaMemcpyAsync(costs, e->vis_costs_d, (size_t)n * (e->T + 1) * sizeof(float), cudaMemcpyDeviceToHost,
-                           e->stream));
-  CUDA_TRY(cudaMemcpyAsync(crash, e->vis_crash_d, (size_t)n * e->T * sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->side.sample(*e, x0, U_nominal, distribution, sample_idx, n, have_opt ? U_opt : nullptr, outputs, costs, crash);
 }
 
 // Device-side host tail (SURVEY §8 f2; controller.cuh:557-586, 643-663): see nominal_traj_kernel.
@@ -1999,31 +2039,7 @@ int mppib_nominal_trajectory(mppib_engine* e, const float* x0, const float* U, c
     if (!std::isfinite(x0[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "x0[%d] is not finite", i);
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  const size_t n_u = (size_t)e->D * e->TC, n_s = (size_t)e->D * e->T * e->S, n_o = (size_t)e->D * e->T * e->O;
-  if (!e->nom_d)
-    CUDA_TRY(e->nom_d.alloc(n_u + n_s + n_o));
-  if (!e->nom_h)
-    CUDA_TRY(e->nom_h.alloc(n_u + n_s + n_o, cudaHostAllocDefault));
-  const float* u_src = e->reduction.result() + kPartialHeader;  // the optimised sequence where K2 / KX left it
-  int u_stride = e->reduction.pstride();
-  if (U)
-  {
-    if (!e->nom_u_d)
-      CUDA_TRY(e->nom_u_d.alloc(n_u));
-    CUDA_TRY(cudaMemcpyAsync(e->nom_u_d, U, n_u * sizeof(float), cudaMemcpyHostToDevice, e->stream));
-    u_src = e->nom_u_d;
-    u_stride = e->TC;
-  }
-  rc = e->pair->nominal_traj(*e, x0, u_src, u_stride, control_history);
-  if (rc != MPPIB_OK)
-    return rc;
-  CUDA_TRY(cudaMemcpyAsync(e->nom_h, e->nom_d, (n_u + n_s + n_o) * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  if (U_smoothed)
-    memcpy(U_smoothed, e->nom_h, n_u * sizeof(float));
-  memcpy(states, e->nom_h + n_u, n_s * sizeof(float));
-  memcpy(outputs, e->nom_h + n_u + n_s, n_o * sizeof(float));
-  return MPPIB_OK;
+  return e->side.nominal(*e, x0, U, control_history, U_smoothed, states, outputs);
 }
 
 int mppib_set_option(mppib_engine* e, int option, long long value)

@@ -3,7 +3,8 @@ demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
   - an RMPPI engine (quadrotor + QuadrotorMapCost, D = 2): solve, init-eval twice with more candidates the second time, the
     cost map replaced by one with four times the cells, a DDP at the horizon that writes the feedback gains, a longer DDP
     that grows its workspace, the feedback gains freed and set again, a solve after each;
-  - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time;
+  - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time,
+    the device-side roll-forward of the caller's controls and of the solve's result;
   - a ColoredNoise and an NLN engine (the samplers whose spectrum, plan and log-normal planes the noise source owns): solve,
     new sampler parameters, solve, burn_draws, solve;
   - an Autorally engine: solve, new NN weights, solve, a costmap with four times the texels, solve;
@@ -61,6 +62,8 @@ def exercise():
     for n in (8, 256):
         idx = np.concatenate([[-1], np.arange(n - 1)]).astype(np.int32)
         e.sample_trajectories(w.x0[0], w.U0[0], idx, U_opt=U_opt[0])
+    e.nominal_trajectory(w.x0, U_opt, np.zeros((2, 4), np.float32))
+    e.nominal_trajectory(w.x0)
     e.close()
 
     # N * T a multiple of 8192: an NLN draw re-positions the generator after burn_draws only on such a boundary
