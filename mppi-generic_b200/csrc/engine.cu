@@ -136,30 +136,6 @@ static std::vector<PairEntry*>& user_pairs()
   return v;
 }
 
-// ---- helpers ----------------------------------------------------------------------------------------------------
-static int make_tensor_map(mppib_engine& e, float* base, CUtensorMap* out)
-{
-  // 2-D view of the noise buffer: rows = local rollouts, cols = T*C floats (row pitch T*C*4 B, must be 16-B multiple)
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-  if (!fn || qres != cudaDriverEntryPointSuccess)
-    return fail(MPPIB_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t gdim[2] = { (cuuint64_t)e.TC, (cuuint64_t)e.n_local };
-  cuuint64_t gstride[1] = { (cuuint64_t)e.TC * sizeof(float) };
-  cuuint32_t box[2] = { (cuuint32_t)kChunkFloats, (cuuint32_t)e.k1.bx };
-  cuuint32_t estride[2] = { 1, 1 };
-  CUresult r = ((EncodeFn)fn)(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstride, box, estride,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(MPPIB_ERR_CUDA, "cuTensorMapEncodeTiled failed: CUresult %d", (int)r);
-  return MPPIB_OK;
-}
-
 // ---- the noise draw (noise_source.cuh) ----------------------------------------------------------------------------
 // n zeroed floats after room for the offset-alignment lead-in of a library draw (see gen_draw); *out = their start
 static cudaError_t alloc_with_lead(DeviceBuffer<float>& b, size_t n, cudaStream_t s, float** out)
@@ -731,10 +707,10 @@ static int check_ready(mppib_engine* e)
   return MPPIB_OK;
 }
 
-// ---- choice of the rollout kernel (K1) ----------------------------------------------------------------------------
+// ---- the rollout kernel K1 (rollout.cuh) -----------------------------------------------------------------------------
 // The descriptor flags and environment variables that choose K1's form or geometry, for A/B runs and tests of each form.
 // Read once per mppib_create; each rule below validates the values it uses.
-struct K1Overrides
+struct mppib::K1Overrides
 {
   bool no_tma;     // MPPIB_FLAG_NO_TMA / MPPIB_NO_TMA: stage the noise with plain loads, never TMA
   bool nn_tensor;  // MPPIB_FLAG_NN_TENSOR / MPPIB_NN_TENSOR: Autorally network on wgmma (rollout_kernel_nn_tc.cuh)
@@ -752,14 +728,17 @@ struct K1Overrides
   bool stream;
   bool stream_readback;  // MPPIB_STREAM_READBACK: generic streaming form writes its controls back and re-reads them
 };
-static K1Overrides read_k1_overrides(const mppib_desc& desc)
+// The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
+// tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
+// *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that has one, even if NN_MMA then keeps the mma.sync entry.
+int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out, bool* wgmma_asked)
 {
   const char* bx = getenv("MPPIB_BX");
   const char* spw = getenv("MPPIB_SPW");
   const char* spt = getenv("MPPIB_SPT");
   const char* ws_pspw = getenv("MPPIB_WS_PSPW");
   const char* stream = getenv("MPPIB_STREAM");
-  K1Overrides o;
+  K1Overrides& o = *ov;
   o.no_tma = (desc.flags & MPPIB_FLAG_NO_TMA) || getenv("MPPIB_NO_TMA");
   o.nn_tensor = (desc.flags & MPPIB_FLAG_NN_TENSOR) || getenv("MPPIB_NN_TENSOR");
   o.nn_ffma2 = (desc.flags & MPPIB_FLAG_NN_FFMA2) || getenv("MPPIB_NN_FFMA2");
@@ -775,14 +754,7 @@ static K1Overrides read_k1_overrides(const mppib_desc& desc)
   o.stream_set = stream != nullptr;
   o.stream = stream && atoi(stream) != 0;
   o.stream_readback = getenv("MPPIB_STREAM_READBACK") != nullptr;
-  return o;
-}
 
-// The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
-// tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
-// *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that has one, even if NN_MMA then keeps the mma.sync entry.
-static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairEntry** out, bool* wgmma_asked)
-{
   const PairEntry* entry = nullptr;
   for (const auto& p : kPairs)
     if (p.dyn_id == desc.dynamics_id && p.cost_id == desc.cost_id)
@@ -790,15 +762,15 @@ static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairE
   for (const PairEntry* p : user_pairs())  // out-of-tree pairs (mppib_load_plugin / mppib_register_pair)
     if (p->dyn_id == desc.dynamics_id && p->cost_id == desc.cost_id)
       entry = p;
-  *wgmma_asked = entry && entry->has_wgmma && ov.nn_tensor;
+  *wgmma_asked = entry && entry->has_wgmma && o.nn_tensor;
   // Autorally pair: the network runs on register-level mma.sync by default (plugins/nn_mma.cuh). NN_FFMA2 keeps the FFMA2
   // form, NN_TENSOR selects the wgmma kernel (which is built on the FFMA2 entry).
-  if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(ov.nn_ffma2 || ov.nn_tensor) || ov.nn_mma))
+  if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(o.nn_ffma2 || o.nn_tensor) || o.nn_mma))
   {
     // samples per warp of the generic kernel's network (plugins/nn_mma.cuh): 32. Narrower sample groups (MPPIB_SPW = 16 / 8)
     // halve / quarter a warp's tensor work per step, but the step time of a lone warp barely moves: the chain, not the
     // work, is the limit — which the warp-specialised kernel (rollout_kernel_ar_ws.cuh, the default for D == 1) removes instead.
-    const int spw = (ov.spw == 16 || ov.spw == 8) ? ov.spw : 32;
+    const int spw = (o.spw == 16 || o.spw == 8) ? o.spw : 32;
     for (const auto& p : kPairsMma)
       if (p.cost_id == desc.cost_id && p.spw == spw)
         entry = &p;
@@ -806,24 +778,33 @@ static int pick_entry(const mppib_desc& desc, const K1Overrides& ov, const PairE
   // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
   // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network.
   if (entry && desc.dynamics_id == MPPIB_DYN_RACER_LSTM && desc.model_dims[0] == lstm_mma::H &&
-      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !ov.lstm_simt)
+      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt)
     for (const auto& p : kPairsLstmMma)
       if (p.cost_id == desc.cost_id)
         entry = &p;
   if (!entry)
     return fail(MPPIB_ERR_UNSUPPORTED, "no kernel registered for dynamics %d + cost %d", desc.dynamics_id, desc.cost_id);
   // the wgmma kernel (rollout_kernel_nn_tc.cuh) is built for ARStandardCost only: refuse rather than run another kernel
-  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc.cost_id == MPPIB_COST_AR_ROBUST && ov.nn_tensor)
+  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && desc.cost_id == MPPIB_COST_AR_ROBUST && o.nn_tensor)
     return fail(MPPIB_ERR_UNSUPPORTED, "MPPIB_FLAG_NN_TENSOR: the tensor-core Autorally kernel supports ARStandardCost only, "
                                        "not ARRobustCost");
   *out = entry;
   return MPPIB_OK;
 }
 
+// resident CTAs per SM of the generic kernel's streaming form (registers, threads and shared memory all count), for
+// choose_k1 before it takes that form; the rule queries the write-back instantiation whatever the engine's write-back
+static int stream_blocks_per_sm(const PairEntry* entry, const K1Plan& plan, int threads, size_t smem)
+{
+  int n = 0;
+  return entry->kernel_attributes(plan, true, true, smem, threads, &n) == MPPIB_OK ? n : 0;
+}
+
 // K1's plan for an engine whose sizes, flags and SM count are set, from its pair entry, the overrides and the device's
-// limits: the generic, SPT = 2, RMPPI, warp-specialised or wgmma kernel, resident or streaming, and bx, threads, grid,
-// shared memory. `wgmma_asked`: NN_TENSOR asks for the wgmma kernel of a pair that has one (pick_entry).
-static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Overrides& ov, bool wgmma_asked, K1Plan* out)
+// limits (max_smem: per block, opted in; smem_per_sm: per multiprocessor): the generic, SPT = 2, RMPPI, warp-specialised or
+// wgmma kernel, resident or streaming, and bx, threads, grid, shared memory. `wgmma_asked`: see Rollout::pick.
+static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Overrides& ov, bool wgmma_asked, int nchunks,
+                     int max_smem, int smem_per_sm, K1Plan* out)
 {
   // One thread per sample; bx samples per CTA, whole-horizon noise tile resident in shared memory. The rollout is bound by
   // the T-step dependency chain, so a CTA takes the same time whatever its width: the block width is chosen to put every CTA
@@ -831,9 +812,6 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
   // warps contending per scheduler); 64 if several waves are unavoidable.
   const mppib_desc& desc = e.desc;
   const int num_sms = e.num_sms;
-  int max_smem = 0, smem_per_sm = 0;
-  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, desc.device));
-  CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, desc.device));
   K1Plan p;
   p.D = e.D;
   const bool tma_ok = !ov.no_tma && e.TC % 4 == 0;
@@ -858,7 +836,7 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
     const int dyn_floats = ws ? ar_ws::sharedFloats(b) : entry->dyn_shared_floats(desc.model_dims, b);
     return (int)rollout_smem_layout(b, chunks, e.D, e.TC, dyn_floats, entry->cost_shared_floats(e.T)).total;
   };
-  auto smem_for = [&](int b) { return layout(b, e.nchunks); };
+  auto smem_for = [&](int b) { return layout(b, nchunks); };
   const int unit = ws ? 32 : entry->spw * spt;  // samples per warp of threads
   const int max_bx = ws ? 32 * ar_ws::maxGroups(p.ws_pspw) : entry->max_block_threads / 32 * unit;  // samples per CTA (__launch_bounds__)
   auto threads_for = [&](int b) { return ws ? ws_wpg * b : b / spt * lps; };
@@ -929,7 +907,7 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
     return fail(MPPIB_ERR_SMEM, "noise tile needs %u B of shared memory, device allows %d", p.smem_bytes, max_smem);
   // tensor-core variant of the Autorally pair: fixed 128-sample CTAs (one warpgroup, two m64 wgmma tiles), streaming
   // noise ring. Opt-in: three exposed MMA round trips per step with few warps per SM to cover them.
-  // MPPIB_FLAG_NN_MMA with NN_TENSOR keeps the mma.sync entry (pick_entry), which has no wgmma kernel: the form chosen
+  // MPPIB_FLAG_NN_MMA with NN_TENSOR keeps the mma.sync entry (Rollout::pick), which has no wgmma kernel: the form chosen
   // above launches, at the wgmma kernel's width and shared memory (streaming only in the warp-specialised form). This is
   // deliberate: the flag combination keeps the launch it has always had.
   const bool wgmma_width = wgmma_asked && e.D == 1 && tma_ok;
@@ -955,12 +933,12 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
     const bool env_bx_ok = ov.bx >= unit && ov.bx <= max_bx && (ov.bx % unit) == 0;
     const int sbx = ws ? ((ws_one_wave && !ov.bx_set) ? ws_one_wave : bx) : (env_bx_ok ? ov.bx : 64);
     const int sm_str = layout(sbx, ring);
-    const bool auto_ok = tma_ok && e.nchunks > ring;
+    const bool auto_ok = tma_ok && nchunks > ring;
     if ((ws || (auto_ok && !e.rmppi && !wgmma_width && spt == 1)) && sm_str <= max_smem)
     {
       // the generic kernel asks the occupancy API (registers count too); the warp-specialised one's budget is fixed
       const int per_sm_str = ws ? std::max(1, ctas_per_sm(sbx, sm_str))
-                                : entry->stream_blocks_per_sm(p, threads_for(sbx), (size_t)sm_str);
+                                : stream_blocks_per_sm(entry, p, threads_for(sbx), (size_t)sm_str);
       if (per_sm_str > 0)
       {
         const long waves_res = waves(bx, std::max(1, ctas_per_sm(bx, smem_for(bx))));
@@ -970,7 +948,7 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
         if (want)
         {
           p.stream = true;
-          // A/B: the round-1 form, controls written back and re-read by the epilogue (mppib_create turns write-back on)
+          // A/B: the round-1 form, controls written back and re-read by the epilogue (Rollout::create turns write-back on)
           p.stream_readback = !ws && ov.stream_readback;
           bx = sbx;
           p.smem_bytes = (uint32_t)sm_str;
@@ -988,6 +966,104 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
   p.use_tma = tma_ok;
   *out = p;
   return MPPIB_OK;
+}
+
+// 2-D view of a noise buffer: rows = local rollouts, cols = T*C floats (row pitch T*C*4 B, must be 16-B multiple); box =
+// one 32-column slab of bx rows
+static int make_tensor_map(float* base, int TC, int n_local, int bx, CUtensorMap* out)
+{
+  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+  if (!fn || qres != cudaDriverEntryPointSuccess)
+    return fail(MPPIB_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
+  cuuint64_t gdim[2] = { (cuuint64_t)TC, (cuuint64_t)n_local };
+  cuuint64_t gstride[1] = { (cuuint64_t)TC * sizeof(float) };
+  cuuint32_t box[2] = { (cuuint32_t)kChunkFloats, (cuuint32_t)bx };
+  cuuint32_t estride[2] = { 1, 1 };
+  CUresult r = ((EncodeFn)fn)(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstride, box, estride,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(MPPIB_ERR_CUDA, "cuTensorMapEncodeTiled failed: CUresult %d", (int)r);
+  return MPPIB_OK;
+}
+
+int Rollout::create(const mppib_engine& e, const PairEntry* entry, const K1Overrides& ov, bool wgmma_asked)
+{
+  pair_ = entry;
+  stream_ = e.stream;
+  D_ = e.D;
+  n_local_ = e.n_local;
+  TC_ = e.TC;
+  nchunks_ = (e.TC + kChunkFloats - 1) / kChunkFloats;
+  if (nchunks_ > kMaxChunks)
+    return fail(MPPIB_ERR_UNSUPPORTED, "T*C = %d exceeds %d", e.TC, kMaxChunks * kChunkFloats);
+  int max_smem = 0, smem_per_sm = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, e.desc.device));
+  CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, e.desc.device));
+  if (int rc = choose_k1(e, entry, ov, wgmma_asked, nchunks_, max_smem, smem_per_sm, &plan_))
+    return rc;
+  const bool writeback = e.rmppi || (e.desc.flags & MPPIB_FLAG_WRITEBACK_CONTROLS) || plan_.stream_readback;
+  CUDA_TRY(costs_.alloc((size_t)D_ * n_local_));
+  if (writeback)
+    CUDA_TRY(controls_.alloc((size_t)D_ * n_local_ * TC_));
+  if (plan_.use_tma)
+    for (int i = 0; i < 2; i++)
+      if (int rc = make_tensor_map(e.noise.buffer(i), TC_, n_local_, plan_.bx, &tmap_[i]))
+        return rc;
+  return entry->kernel_attributes(plan_, plan_.stream, writeback, plan_.smem_bytes, plan_.threads, nullptr);
+}
+
+int Rollout::launch(mppib_engine& e, const float* x0, const float* U, int opt_stride, int iter) const
+{
+  return pair_->launch(e, x0, U, opt_stride, iter);
+}
+
+int Rollout::read_costs(float* host) const
+{
+  CUDA_TRY(cudaMemcpyAsync(host, costs_, (size_t)D_ * n_local_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
+}
+
+int Rollout::read_controls(float* host) const
+{
+  if (!controls_)
+    return fail(MPPIB_ERR_STATE, "engine was created without MPPIB_FLAG_WRITEBACK_CONTROLS");
+  CUDA_TRY(cudaMemcpyAsync(host, controls_, (size_t)D_ * n_local_ * TC_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
+}
+
+int Rollout::weights(float* host, const float* result, int pstride, float lambda)
+{
+  const size_t n = (size_t)D_ * n_local_;
+  if (!weights_)
+    CUDA_TRY(weights_.alloc(n));
+  const dim3 grid((n_local_ + 255) / 256 > 1024 ? 1024 : (n_local_ + 255) / 256, D_);
+  weights_kernel<<<grid, 256, 0, stream_>>>(costs_, result, n_local_, pstride, (float)(1.0 / lambda), weights_);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(host, weights_, n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
+}
+
+int Rollout::set_l2_flush(long long bytes)
+{
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  l2_flush_.reset();
+  if (bytes > 0)  // exactly that many bytes: a larger buffer would change what is flushed
+    CUDA_TRY(l2_flush_.alloc((size_t)bytes));
+  return MPPIB_OK;
+}
+
+cudaError_t Rollout::flush_l2() const
+{
+  return l2_flush_ ? cudaMemsetAsync(l2_flush_, 0, l2_flush_.capacity(), stream_) : cudaSuccess;
 }
 
 // =================================================================================================================
@@ -1095,7 +1171,6 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   if (!out || !desc)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   *out = nullptr;
-  const K1Overrides ov = read_k1_overrides(*desc);
   if (desc->num_rollouts <= 0 || desc->num_timesteps <= 0)
     return fail(MPPIB_ERR_INVALID_ARG, "num_rollouts and num_timesteps must be positive");
   if (desc->num_distributions < 1 || desc->num_distributions > MPPIB_MAX_DISTRIBUTIONS)
@@ -1123,9 +1198,10 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     if (desc->num_distributions != 1)
       return fail(MPPIB_ERR_UNSUPPORTED, "RacerDubinsElevationLSTMSteering is built for num_distributions == 1 only");
   }
+  K1Overrides ov;
   const PairEntry* entry = nullptr;
   bool wgmma_asked = false;
-  if (int rc = pick_entry(*desc, ov, &entry, &wgmma_asked))
+  if (int rc = Rollout::pick(*desc, &ov, &entry, &wgmma_asked))
     return rc;
 
   int ndev = 0;
@@ -1149,17 +1225,12 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   e->N = desc->num_rollouts;
   e->T = desc->num_timesteps;
   e->TC = e->T * e->C;
-  e->pair = entry;
   e->rmppi = (desc->flags & MPPIB_FLAG_RMPPI) != 0;
   if (e->rmppi && desc->num_distributions != 2)
     return fail(MPPIB_ERR_INVALID_ARG, "MPPIB_FLAG_RMPPI needs num_distributions == 2 (nominal, real)");
-  e->writeback = e->rmppi || (desc->flags & MPPIB_FLAG_WRITEBACK_CONTROLS) != 0;
 
   if (e->D * e->TC > kMaxMeanFloats)
     return fail(MPPIB_ERR_UNSUPPORTED, "D*T*C = %d exceeds %d", e->D * e->TC, kMaxMeanFloats);
-  e->nchunks = (e->TC + kChunkFloats - 1) / kChunkFloats;
-  if (e->nchunks > kMaxChunks)
-    return fail(MPPIB_ERR_UNSUPPORTED, "T*C = %d exceeds %d", e->TC, kMaxChunks * kChunkFloats);
 
   // rollout sharding (SURVEY §8e): contiguous slices, remainder to the last rank
   const int per = e->N / world;
@@ -1169,10 +1240,6 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return fail(MPPIB_ERR_INVALID_ARG, "rank %d of %d has no rollouts (N=%d)", desc->rank, world, e->N);
 
   CUDA_TRY(cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, desc->device));
-  if (int rc = choose_k1(*e, entry, ov, wgmma_asked, &e->k1))
-    return rc;
-  if (e->k1.stream_readback)
-    e->writeback = true;
 
   int prio_lo = 0, prio_hi = 0;
   CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
@@ -1185,19 +1252,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   e->feedback.create(e->S, e->C, e->T, e->stream);
   if (int rc = e->noise.create(e->desc, e->N, e->n_offset, e->n_local, e->T, e->C, e->num_sms, e->stream, prio_lo))
     return rc;
-  CUDA_TRY(e->costs_d.alloc((size_t)e->D * e->n_local));
-  if (int rc = e->reduction.create(e->D, e->TC, e->k1.grid, world, desc->rank, e->stream))
+  if (int rc = e->rollout.create(*e, entry, ov, wgmma_asked))
     return rc;
-  if (e->writeback)
-    CUDA_TRY(e->controls_d.alloc((size_t)e->D * e->n_local * e->TC));
+  if (int rc = e->reduction.create(e->D, e->TC, e->rollout.plan().grid, world, desc->rank, e->stream))
+    return rc;
   CUDA_TRY(e->timer.create());
-
-  if (e->k1.use_tma)
-    for (int i = 0; i < 2; i++)
-      if (int rc = make_tensor_map(*e, e->noise.buffer(i), &e->tmap[i]))
-        return rc;
-  if (int rc = entry->prepare(*e))
-    return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
   *out = owner.release();
   return MPPIB_OK;
@@ -1560,7 +1619,7 @@ int mppib_rollout_only(mppib_engine* e, const float* x0, const float* U_in, int 
   if (!x0 || !U_in)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = e->pair->launch(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = e->rollout.launch(*e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -1576,7 +1635,7 @@ int mppib_reduce_only(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
   if (!e->solved_once)
     return fail(MPPIB_ERR_STATE, "no rollout has been run yet");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = e->reduction.enqueue(false, e->costs_d, e->controls_d, e->n_local, e->lambda);
+  rc = e->reduction.enqueue(false, e->rollout.costs(), e->rollout.controls(), e->n_local, e->lambda);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -1639,10 +1698,9 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
   int rc = e->noise.draw(optimization_stride);
   if (rc != MPPIB_OK)
     return rc;
-  if (e->l2_flush_d)
-    CUDA_TRY(cudaMemsetAsync(e->l2_flush_d, 0, e->l2_flush_d.capacity(), e->stream));
+  CUDA_TRY(e->rollout.flush_l2());
   CUDA_TRY(e->timer.mark(1, e->stream));
-  rc = e->pair->launch(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = e->rollout.launch(*e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   rc = e->noise.prefetch();
@@ -1650,7 +1708,8 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
     return rc;
   CUDA_TRY(e->timer.mark(2, e->stream));
   // a timed solve records an event between K1 and K2: no PDL then
-  rc = e->reduction.enqueue(/*after_k1=*/!e->timer.timed(), e->costs_d, e->controls_d, e->n_local, e->lambda);
+  rc = e->reduction.enqueue(/*after_k1=*/!e->timer.timed(), e->rollout.costs(), e->rollout.controls(), e->n_local,
+                            e->lambda);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(e->noise.read_by_kernel());  // K1 read it; recorded after K2, so nothing sits between K1 and PDL's K2
@@ -1745,7 +1804,7 @@ int mppib_set_tsallis(mppib_engine* e, float gamma, float r)
 {
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
-  return e->reduction.set_tsallis(gamma, r, e->controls_d != nullptr);
+  return e->reduction.set_tsallis(gamma, r, e->rollout.controls() != nullptr);
 }
 
 // ---- the feedback controller (feedback.cuh) ---------------------------------------------------------------------------
@@ -1822,7 +1881,7 @@ int Feedback::compute(mppib_engine& e, int T, const float* x0, const float* x_ta
   CUDA_TRY(cudaMemcpyAsync(ws + L.ut, u_target, (size_t)T * C_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
   // computeFeedback(x0, goal_traj, control_traj) starts DDP::run from control_traj, the control targets (ddp.cu:103-104)
   CUDA_TRY(cudaMemcpyAsync(ws + L.u, u_target, (size_t)T * C_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
-  if (int rc = e.pair->ddp(e, T, x0, to_rmppi ? gains_.get() : nullptr))
+  if (int rc = e.rollout.pair().ddp(e, T, x0, to_rmppi ? gains_.get() : nullptr))
     return rc;
   int status = 0;
   CUDA_TRY(cudaMemcpyAsync(&status, status_, sizeof(int), cudaMemcpyDeviceToHost, stream_));
@@ -1868,7 +1927,7 @@ int mppib_ddp_feedback(mppib_engine* e, int T, const float* x0, const float* x_t
 {
   if (!e || !x0 || !x_target || !u_target)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (!e->pair->ddp)
+  if (!e->rollout.pair().ddp)
     return fail(MPPIB_ERR_UNSUPPORTED, "dynamics %d has no analytic Jacobian (computeGrad): no DDP kernel is built for it",
                 e->desc.dynamics_id);
   if (T < 2)
@@ -1907,7 +1966,7 @@ int SideRollouts::init_eval(mppib_engine& e, const float* candidates, const int*
   CUDA_TRY(cudaMemcpyAsync(eval_strides_, strides, (size_t)K * sizeof(int), cudaMemcpyHostToDevice, e.stream));
   if (int rc = e.noise.draw(opt_stride))  // sampler_->generateSamples(stride, 0, gen_) (:595)
     return rc;
-  if (int rc = e.pair->init_eval(e, K, samples, U_nominal, opt_stride))
+  if (int rc = e.rollout.pair().init_eval(e, K, samples, U_nominal, opt_stride))
     return rc;
   CUDA_TRY(e.noise.read_by_kernel());  // the kernel above read the noise: later draws into its buffer wait for it
   CUDA_TRY(cudaMemcpyAsync(costs_out, eval_costs_, total * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
@@ -1930,7 +1989,7 @@ int SideRollouts::sample(mppib_engine& e, const float* x0, const float* U_nomina
     CUDA_TRY(vis_opt_.reserve((size_t)e.TC, e.stream));
     CUDA_TRY(cudaMemcpyAsync(vis_opt_, U_opt, (size_t)e.TC * sizeof(float), cudaMemcpyHostToDevice, e.stream));
   }
-  if (int rc = e.pair->sampled_traj(e, x0, U_nominal, distribution, n))
+  if (int rc = e.rollout.pair().sampled_traj(e, x0, U_nominal, distribution, n))
     return rc;
   CUDA_TRY(cudaMemcpyAsync(outputs, vis_outputs_, n_out * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
   CUDA_TRY(cudaMemcpyAsync(costs, vis_costs_, n_cost * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
@@ -1956,7 +2015,7 @@ int SideRollouts::nominal(mppib_engine& e, const float* x0, const float* U, cons
     nom_src_ = nom_u_;
     nom_stride_ = e.TC;
   }
-  if (int rc = e.pair->nominal_traj(e, x0, history))
+  if (int rc = e.rollout.pair().nominal_traj(e, x0, history))
     return rc;
   CUDA_TRY(cudaMemcpyAsync(nom_h_, nom_, n * sizeof(float), cudaMemcpyDeviceToHost, e.stream));
   CUDA_TRY(cudaStreamSynchronize(e.stream));
@@ -1997,7 +2056,7 @@ int mppib_sample_trajectories(mppib_engine* e, const float* x0, const float* U_n
     return fail(MPPIB_ERR_INVALID_ARG, "bad argument");
   if (distribution < 0 || distribution >= e->D)
     return fail(MPPIB_ERR_INVALID_ARG, "distribution %d out of range [0, %d)", distribution, e->D);
-  if (!e->writeback || !e->controls_d)
+  if (!e->rollout.controls())
     return fail(MPPIB_ERR_STATE, "sampled trajectories re-roll the written-back controls: create the engine with "
                                  "MPPIB_FLAG_WRITEBACK_CONTROLS");
   if (e->rmppi)
@@ -2054,11 +2113,7 @@ int mppib_set_option(mppib_engine* e, int option, long long value)
   switch (option)
   {
     case MPPIB_OPT_L2_FLUSH_BYTES:
-      CUDA_TRY(cudaStreamSynchronize(e->stream));
-      e->l2_flush_d.reset();
-      if (value > 0)  // exactly that many bytes: a larger buffer would change what is flushed
-        CUDA_TRY(e->l2_flush_d.alloc((size_t)value));
-      return MPPIB_OK;
+      return e->rollout.set_l2_flush(value);
   }
   return fail(MPPIB_ERR_INVALID_ARG, "unknown option %d", option);
 }
@@ -2068,10 +2123,7 @@ int mppib_get_costs(mppib_engine* e, float* host_costs)
   if (!e || !host_costs)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  CUDA_TRY(cudaMemcpyAsync(host_costs, e->costs_d, (size_t)e->D * e->n_local * sizeof(float), cudaMemcpyDeviceToHost,
-                           e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->rollout.read_costs(host_costs);
 }
 
 int mppib_get_noise(mppib_engine* e, float* host_eps)
@@ -2089,13 +2141,8 @@ int mppib_get_samples(mppib_engine* e, float* host_samples)
 {
   if (!e || !host_samples)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
-  if (!e->writeback)
-    return fail(MPPIB_ERR_STATE, "engine was created without MPPIB_FLAG_WRITEBACK_CONTROLS");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  CUDA_TRY(cudaMemcpyAsync(host_samples, e->controls_d, (size_t)e->D * e->n_local * e->TC * sizeof(float),
-                           cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->rollout.read_controls(host_samples);
 }
 
 int mppib_get_weights(mppib_engine* e, float* host_weights)
@@ -2105,16 +2152,7 @@ int mppib_get_weights(mppib_engine* e, float* host_weights)
   if (!e->solved_once)
     return fail(MPPIB_ERR_STATE, "no solve has been run yet");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  const size_t n = (size_t)e->D * e->n_local;
-  if (!e->weights_d)
-    CUDA_TRY(e->weights_d.alloc(n));
-  const dim3 grid((e->n_local + 255) / 256 > 1024 ? 1024 : (e->n_local + 255) / 256, e->D);
-  weights_kernel<<<grid, 256, 0, e->stream>>>(e->costs_d, e->reduction.result(), e->n_local, e->reduction.pstride(),
-                                              (float)(1.0 / e->lambda), e->weights_d);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(host_weights, e->weights_d, n * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-  CUDA_TRY(cudaStreamSynchronize(e->stream));
-  return MPPIB_OK;
+  return e->rollout.weights(host_weights, e->reduction.result(), e->reduction.pstride(), e->lambda);
 }
 
 int mppib_enable_timing(mppib_engine* e, int enable)
@@ -2137,14 +2175,15 @@ int mppib_get_launch_info(mppib_engine* e, int* grid, int* block, int* smem_byte
 {
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
+  const K1Plan& k1 = e->rollout.plan();
   if (grid)
-    *grid = e->k1.grid;
+    *grid = k1.grid;
   if (block)
-    *block = e->k1.threads;
+    *block = k1.threads;
   if (smem_bytes)
-    *smem_bytes = (int)e->k1.smem_bytes;
+    *smem_bytes = (int)k1.smem_bytes;
   if (uses_tma)
-    *uses_tma = e->k1.use_tma ? 1 : 0;
+    *uses_tma = k1.use_tma ? 1 : 0;
   if (kernels_per_solve)  // [K0] + K1 + K2 (+ K2'); cuRAND's own launches are not counted
     *kernels_per_solve = ((e->desc.world_size > 1) ? 3 : 2) + (e->noise.own_kernel() ? 1 : 0);
   return MPPIB_OK;

@@ -8,15 +8,15 @@
  * the side kernels (init-eval, sampled trajectories, the roll-forward: side_rollout_kernels.cuh) and the DDP kernel for it
  * — and handed to the engine with mppib_register_pair(); see plugins_example/ and INTEGRATION.md §E. The plugin library
  * and libmppi_b200.so must be built from the same source revision (kEngineAbi is checked at registration).
- * An engine keeps a pointer to its pair's entry and one K1Plan: the form and geometry of its rollout kernel, chosen once
- * by engine.cu's choose_k1. Pair<>::kernel maps the plan's form to the instantiation that launches.
- * Five parts of the engine have an owner of their own, declared in their headers and defined in engine.cu: the noise
- * draw (NoiseSource, noise_source.cuh), the merge from K1's block partials to the result record (Reduction,
- * reduction.cuh), the model's blobs: parameters, weights and maps (ModelParams, model_params.cuh), the feedback
- * controller: DDP's weights and workspace and RMPPI's gains (Feedback, feedback.cuh), and the side rollouts' scratch
- * (SideRollouts, side_rollouts.cuh). K1 reads the current noise buffer, writes the partials and takes the model's blobs and
- * the gains through their accessors; the DDP launch reads the weights, the side launches their inputs and outputs. The
- * stage timing of a solve is a sixth, StageTimer, declared below.
+ * Six parts of the engine have an owner of their own, declared in their headers and defined in engine.cu: the noise
+ * draw (NoiseSource, noise_source.cuh), K1 itself: its pair entry, its K1Plan (the form and geometry, chosen once), the
+ * tensor maps, costs and written-back controls (Rollout, rollout.cuh), the merge from K1's block partials to the result
+ * record (Reduction, reduction.cuh), the model's blobs: parameters, weights and maps (ModelParams, model_params.cuh), the
+ * feedback controller: DDP's weights and workspace and RMPPI's gains (Feedback, feedback.cuh), and the side rollouts'
+ * scratch (SideRollouts, side_rollouts.cuh). Pair<>::kernel maps the plan's form to the instantiation that launches. K1
+ * reads the current noise buffer, its plan and buffers, writes the partials and takes the model's blobs and the gains
+ * through their accessors; the DDP launch reads the weights, the side launches their inputs and outputs. The stage timing
+ * of a solve is a seventh, StageTimer, declared below.
  */
 #pragma once
 #include <cuda.h>
@@ -44,6 +44,7 @@
 #include "plugins/costs.cuh"
 #include "plugins/dynamics.cuh"
 #include "reduction.cuh"
+#include "rollout.cuh"
 #include "rollout_kernel.cuh"
 #include "rollout_kernel_ar_ws.cuh"
 #include "rollout_kernel_nn_tc.cuh"
@@ -78,35 +79,6 @@ static inline int fail(int status, const char* fmt, A... a)
 
 using namespace mppib;
 
-// ---- K1's form and geometry, chosen once per engine by mppib_create (engine.cu: choose_k1) ------------------------
-enum class K1Form
-{
-  Generic,      // rollout_kernel.cuh, one sample per thread
-  GenericSpt2,  // rollout_kernel.cuh, two samples per thread (MPPIB_SPT = 2)
-  Rmppi,        // rollout_kernel.cuh, RMPPI: nominal and real system (MPPIB_FLAG_RMPPI)
-  WarpSpec,     // rollout_kernel_ar_ws.cuh: Autorally pair, producer and consumer warps
-  Wgmma,        // rollout_kernel_nn_tc.cuh: Autorally pair, the network on wgmma tensor cores
-};
-struct K1Plan
-{
-  K1Form form = K1Form::Generic;
-  int D = 1;                     // distributions per sample, as the generic kernel is instantiated
-  bool stream = false;           // noise slabs through a ring, controls kept in HBM (STREAM; generic or warp-specialised)
-  bool stream_readback = false;  // generic streaming form, A/B (MPPIB_STREAM_READBACK): weighted sum from written-back controls
-  int ws_pspw = 16;  // warp-specialised kernel: samples per producer warp; threads per CTA = bx * (32 / ws_pspw + 1)
-  int spt = 1;       // samples per thread; generic kernel: threads per CTA = bx / spt * lps
-  int lps = 1;       // lanes per sample = 32 / DYN::SAMPLES_PER_WARP (rollout_kernel.cuh: SPW)
-  int ring = 2;      // noise slabs in the generic streaming form's ring
-  int bx = 64;       // samples (noise-tile rows) per CTA
-  int threads = 0;   // threads per CTA
-  int grid = 0;
-  uint32_t smem_bytes = 0;
-  bool use_tma = false;
-  int dyn_shared_floats = 0;  // the dynamics' shared floats for a CTA of bx samples
-};
-
-struct PairEntry;
-
 // ---- stage timing (mppib_enable_timing / mppib_get_timing; definitions in engine.cu) -----------------------------------
 // Events at the start of a solve, after the noise draw, after K1 and after K2. Whether a solve is timed is decided once, as
 // it is enqueued; a drained solve adds a sample only if it was timed and timing is still on. With several solves in flight
@@ -140,16 +112,10 @@ struct mppib_engine
   Stream stream;  // the solve's stream: the engine's own, or mppib_desc.stream borrowed
 
   mppib_desc desc{};
-  // the (dynamics, cost) pair's kernels and sizes: a built-in entry is static, and a registered one is never freed
-  // (mppib_register_pair), so the pointer outlives the engine
-  const PairEntry* pair = nullptr;
-  K1Plan k1;
   int S = 0, C = 0, O = 0, D = 1;
   int N = 0, T = 0, TC = 0;
   int n_local = 0, n_offset = 0;
-  int nchunks = 0;
   int num_sms = 0;  // multiprocessors of the device (grid-stride kernels launch up to 16 CTAs per SM)
-  bool writeback = false;
   bool rmppi = false;  // MPPIB_FLAG_RMPPI
 
   // solver scalars
@@ -157,17 +123,10 @@ struct mppib_engine
 
   ModelParams model;  // the dynamics and cost blobs, weights and maps (model_params.cuh)
   NoiseSource noise;  // K0 / K0c / NLN draw, its sampler parameters, two buffers and prefetch (noise_source.cuh)
+  Rollout rollout;    // K1: pair entry, plan, tensor maps, costs and written-back controls, weights, L2 flush (rollout.cuh)
   Feedback feedback;  // DDP's weights, workspace and status, RMPPI's gains and value-function threshold (feedback.cuh)
   SideRollouts side;  // init-eval, sampled trajectories and the device-side roll-forward (side_rollouts.cuh)
-
-  // device buffers
-  DeviceBuffer<float> costs_d;        // [D][n_local]
-  DeviceBuffer<float> controls_d;     // optional [D][n_local][T][C]
-  DeviceBuffer<float> weights_d;      // lazily allocated for mppib_get_weights
-  DeviceBuffer<unsigned char> l2_flush_d;  // optional: all of it is written between K0 and K1 to evict the noise from L2
-  int pending = 0;               // solves enqueued and not yet waited for
-
-  CUtensorMap tmap[2]{};  // K1's TMA view of noise.buffer(i) (its box is K1's block width)
+  int pending = 0;    // solves enqueued and not yet waited for
 
   // K1's block partials, K2 and the cross-rank merge, the result record, Tsallis weights, NCCL and KX (reduction.cuh)
   Reduction reduction;
@@ -309,57 +268,49 @@ struct Pair
     fail(MPPIB_ERR_UNSUPPORTED, "this dynamics model is built for num_distributions == 1 only");
     return nullptr;
   }
-  // resident CTAs per SM of the generic kernel's streaming form (registers, threads and shared memory all count), for
-  // choose_k1 before it takes that form; the rule queries the write-back instantiation whatever the engine's write-back
-  static int stream_blocks_per_sm(const K1Plan& plan, int threads, size_t smem)
+  // Sets the dynamic shared memory limit of kernel(k, stream, wb) to `smem` and, with blocks_per_sm, asks how many CTAs
+  // of `threads` threads are resident per SM. Runs in the module that holds the kernels: a plugin library links a CUDA
+  // runtime of its own, and only that one knows its kernels.
+  static int kernel_attributes(const K1Plan& k, bool stream, bool wb, size_t smem, int threads, int* blocks_per_sm)
   {
-    const Kernel k = kernel(plan, true, true);
-    int n = 0;
-    if (!k)
-      return 0;
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, threads, smem) != cudaSuccess)
-    {
-      cudaGetLastError();
-      return 0;
-    }
-    return n;
-  }
-  static int prepare(mppib_engine& e)
-  {
-    const Kernel k = kernel(e.k1, e.k1.stream, e.writeback);
-    if (!k)
+    const Kernel f = kernel(k, stream, wb);
+    if (!f)
       return MPPIB_ERR_UNSUPPORTED;
-    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e.k1.smem_bytes));
+    CUDA_TRY(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (blocks_per_sm)
+      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, f, threads, smem));
     return MPPIB_OK;
   }
 
   static int launch(mppib_engine& e, const float* x0, const float* U_in, int opt_stride, int iter)
   {
     static_assert(sizeof(Args) < 30000, "kernel parameter block too large");
+    const Rollout& r = e.rollout;
+    const K1Plan& k = r.plan();
     Args a;
     fill_pair_args(a, e, iter);
     a.eps = e.noise.eps();
-    a.costs = e.costs_d;
+    a.costs = r.costs();
     a.partials = e.reduction.partials();
     a.headers = e.reduction.headers();
-    a.controls_out = e.writeback ? e.controls_d.get() : nullptr;
+    a.controls_out = r.controls();
     a.n_local = e.n_local;
     a.n_offset = e.n_offset;
     a.T = e.T;
-    a.nchunks = e.nchunks;
+    a.nchunks = r.nchunks();
     a.pstride = e.reduction.pstride();
     a.opt_stride = opt_stride;
-    a.use_tma = e.k1.use_tma ? 1 : 0;
-    a.dyn_shared_floats = e.k1.dyn_shared_floats;
-    a.ring = e.k1.stream ? e.k1.ring : 0;
-    a.stream_readback = e.k1.stream_readback ? 1 : 0;
+    a.use_tma = k.use_tma ? 1 : 0;
+    a.dyn_shared_floats = k.dyn_shared_floats;
+    a.ring = k.stream ? k.ring : 0;
+    a.stream_readback = k.stream_readback ? 1 : 0;
     a.fb_gains = e.feedback.gains();
     a.value_func_threshold = e.feedback.threshold();
     a.lambda_inv = (float)(1.0 / e.lambda);  // mppi_controller.cu:201-202: 1.0 / lambda in double, narrowed
     memcpy(a.x0, x0, sizeof(float) * e.D * e.S);
     memcpy(a.means, U_in, sizeof(float) * e.D * e.TC);
-    kernel(e.k1, e.k1.stream, e.writeback)<<<e.k1.grid, e.k1.threads, e.k1.smem_bytes, e.stream>>>(a, e.tmap[e.noise.current()]);
+    kernel(k, k.stream, r.controls() != nullptr)<<<k.grid, k.threads, k.smem_bytes, e.stream>>>(
+        a, r.tensor_map(e.noise.current()));
     CUDA_TRY(cudaGetLastError());
     return MPPIB_OK;
   }
@@ -404,7 +355,7 @@ static int sampled_traj_launch(mppib_engine& e, const float* x0, const float* U_
 {
   SampledTrajArgs<DYN, COST> a;
   fill_pair_args(a, e, 0);
-  a.controls = e.controls_d + (size_t)distribution * e.n_local * e.TC;
+  a.controls = e.rollout.controls() + (size_t)distribution * e.n_local * e.TC;
   a.opt = e.side.sample_opt();
   a.sample_idx = e.side.sample_idx();
   a.outputs = e.side.sample_outputs();
@@ -496,9 +447,9 @@ struct PairEntry
   bool has_wgmma;      // Pair<>::kHasTensorCoreVariant: K1Form::Wgmma is built for this pair
   int (*cost_shared_floats)(int);
   int (*launch)(mppib_engine&, const float*, const float*, int, int);
-  int (*prepare)(mppib_engine&);  // sets K1's function attributes
+  // Pair<>::kernel_attributes: K1's shared memory limit and occupancy, for a plan, streaming form and write-back
+  int (*kernel_attributes)(const K1Plan&, bool stream, bool wb, size_t smem, int threads, int* blocks_per_sm);
   int (*init_eval)(mppib_engine&, int, int, const float*, int);
-  int (*stream_blocks_per_sm)(const K1Plan&, int, size_t);
   int (*sampled_traj)(mppib_engine&, const float*, const float*, int, int);
   int (*nominal_traj)(mppib_engine&, const float*, const float*);
   int (*ddp)(mppib_engine&, int, const float*, float*);  // null: the dynamics have no analytic Jacobian (HAS_GRAD)
@@ -521,9 +472,8 @@ constexpr PairEntry make_entry(int dyn_id, int cost_id)
                     Pair<DYN, COST>::kHasTensorCoreVariant,
                     &COST::sharedFloats,
                     &Pair<DYN, COST>::launch,
-                    &Pair<DYN, COST>::prepare,
+                    &Pair<DYN, COST>::kernel_attributes,
                     &init_eval_launch<typename DYN::AuxDyn, COST>,
-                    &Pair<DYN, COST>::stream_blocks_per_sm,
                     &sampled_traj_launch<typename DYN::AuxDyn, COST>,
                     &nominal_traj_launch<typename DYN::AuxDyn>,
                     ddp_launcher<typename DYN::AuxDyn>() };
@@ -536,8 +486,8 @@ constexpr PairEntry make_entry(int dyn_id, int cost_id)
 inline unsigned engine_abi()
 {
   using Slots = void (*)(decltype(PairEntry::dyn_shared_floats), decltype(PairEntry::cost_shared_floats),
-                         decltype(PairEntry::launch), decltype(PairEntry::prepare), decltype(PairEntry::init_eval),
-                         decltype(PairEntry::stream_blocks_per_sm), decltype(PairEntry::sampled_traj),
+                         decltype(PairEntry::launch), decltype(PairEntry::kernel_attributes),
+                         decltype(PairEntry::init_eval), decltype(PairEntry::sampled_traj),
                          decltype(PairEntry::nominal_traj), decltype(PairEntry::ddp));
   unsigned h = (unsigned)(sizeof(mppib_engine) * 131u + sizeof(PairEntry) * 7u + sizeof(SamplerArgs));
   for (const char* c = typeid(Slots).name(); *c; c++)

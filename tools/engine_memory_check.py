@@ -4,7 +4,8 @@ demand has done so (csrc/device_resources.cuh: DeviceBuffer::reserve / reset):
     cost map replaced by one with four times the cells, a DDP at the horizon that writes the feedback gains, a longer DDP
     that grows its workspace, the feedback gains freed and set again, a solve after each;
   - a Vanilla engine with written-back controls: solve, sampled trajectories twice with more samples the second time,
-    the device-side roll-forward of the caller's controls and of the solve's result;
+    the device-side roll-forward of the caller's controls and of the solve's result, the importance weights (a buffer made
+    on first use), and an L2 flush set, grown and set to 0, then a solve;
   - a ColoredNoise and an NLN engine (the samplers whose spectrum, plan and log-normal planes the noise source owns): solve,
     new sampler parameters, solve, burn_draws, solve;
   - an Autorally engine: solve, new NN weights, solve, a costmap with four times the texels, solve;
@@ -64,6 +65,10 @@ def exercise():
         e.sample_trajectories(w.x0[0], w.U0[0], idx, U_opt=U_opt[0])
     e.nominal_trajectory(w.x0, U_opt, np.zeros((2, 4), np.float32))
     e.nominal_trajectory(w.x0)
+    e.get_weights()
+    for nbytes in (1 << 20, 8 << 20, 0):
+        e.set_option(H.OPT_L2_FLUSH_BYTES, nbytes)
+    e.solve(w.x0, w.U0)
     e.close()
 
     # N * T a multiple of 8192: an NLN draw re-positions the generator after burn_draws only on such a boundary
