@@ -7,6 +7,7 @@
  *   mppib_host_slide_controls       Controller::slideControlSequenceHelper      controller.cuh:588-600
  *   mppib_host_output_trajectory    Controller::computeOutputTrajectoryHelper   controller.cuh:643-663
  *   mppib_host_step_lstm / mppib_host_output_trajectory_lstm   the same two for RacerDubinsElevationLSTMSteering
+ *   mppib_host_step_racer_suspension / mppib_host_output_trajectory_racer_suspension   ... for RacerDubinsElevationSuspension
  *   mppib_host_free_energy          mppi::kernels::computeFreeEnergy      include/mppi/core/mppi_common.cu:1065-1081
  *   mppib_host_merge_records        (no reference counterpart: the log-sum-exp merge of rollout shards, SURVEY §8e)
  *   mppib_host_state_cost           the robust costs' and QuadrotorMapCost's host computeStateCost and terms (below)
@@ -60,6 +61,20 @@ int mppib_host_grad_racer_dubins_elevation(const void* dyn_params, const float* 
 int mppib_host_output_trajectory_racer_dubins_elevation(const void* dyn_params, const mppib_elevation_map_header* map,
                                                         const float* x0, const float* u, int T, float dt, float* states,
                                                         float* outputs);
+/* RacerDubinsElevationSuspension (racer_dubins_elevation_suspension_lstm.cu:59-197,420-525, host step): the LSTM model's
+ * network and elevation map in `net` (net->map, NULL = height 0), the normals map (header + width * height float4, NULL =
+ * (0, 0, 1)) apart. The host body differs from the device one (DESIGN §8) in sincosf / sinf / tanf of raw angles and in
+ * its brake clamp [0, -control_rngs_[0].x]. S = 24, O = 28; the LSTM state in `net` is updated in place by the step, and
+ * the trajectory starts from the initial state in the weight blob. */
+int mppib_host_step_racer_suspension(const void* dyn_params, const mppib_host_lstm* net,
+                                     const mppib_elevation_map_header* normals, const float* x, const float* u, float dt,
+                                     float* x_next, float* xdot, float* y);
+int mppib_host_output_trajectory_racer_suspension(const void* dyn_params, const mppib_host_lstm* net,
+                                                  const mppib_elevation_map_header* normals, const float* x0,
+                                                  const float* u, int T, float dt, float* states, float* outputs);
+/* TwoDTextureHelper<float4>::queryTextureAtWorldPose on the host: out4 = the four channels, each by the float map's
+ * formula (mppib_host_elevation_at_world_pose); map NULL: (0, 0, 1, 0). */
+void mppib_host_normals_at_world_pose(const mppib_elevation_map_header* map, float x, float y, float z, float* out4);
 /* LSTMLSTMHelper::initializeLSTM (utils/nn_helpers/lstm_lstm_helper.cu:50-73): the INIT network — an LSTM (input_dim, hidden_dim)
  * with an FNN head on [h; x] (layers {hidden_dim + input_dim, ..., 2 * H_prediction}) — runs over the last init_len columns
  * of a buffer of past inputs, starting from its own initial hidden / cell state; the head's output after the last column is

@@ -26,6 +26,7 @@ enum mppib_dynamics_id
   MPPIB_DYN_RACER_LSTM = 3,        /* dynamics/racer_dubins/racer_dubins_elevation_lstm_steering.cuh S19 C2 O28 */
   MPPIB_DYN_QUADROTOR = 4,         /* dynamics/quadrotor/quadrotor_dynamics.cuh          S13 C4 O13 */
   MPPIB_DYN_RACER_DUBINS_ELEVATION = 5, /* dynamics/racer_dubins/racer_dubins_elevation.cuh  S19 C2 O28 */
+  MPPIB_DYN_RACER_SUSPENSION_LSTM = 6,  /* dynamics/racer_dubins/racer_dubins_elevation_suspension_lstm.cuh S24 C2 O28 */
   MPPIB_DYN_COUNT
 };
 
@@ -131,6 +132,22 @@ typedef struct mppib_racer_lstm_dyn_params
  * model (its steering is first order, racer_dubins.cu:296-304). Map: MPPIB_BLOB_ELEVATION_MAP; no weights. */
 typedef mppib_racer_lstm_dyn_params mppib_racer_dubins_elevation_dyn_params;
 
+/* RacerDubinsElevationSuspension (dynamics/racer_dubins/racer_dubins_elevation_suspension_lstm.cuh:14-64): the LSTM model's
+ * blob followed by RacerDubinsElevationSuspensionParams' own fields. The steering network, model_dims and
+ * MPPIB_BLOB_LSTM_WEIGHTS are exactly the LSTM model's. Maps: MPPIB_BLOB_ELEVATION_MAP (wheel heights, unset = 0) and
+ * MPPIB_BLOB_NORMALS_MAP (terrain normals, unset = (0, 0, 1)), both optional. */
+typedef struct mppib_racer_suspension_dyn_params
+{
+  mppib_racer_lstm_dyn_params base;
+  float spring_k;     /* 14000 N / m */
+  float drag_c;       /* 1000 N s / m */
+  float mass;         /* 1447 kg */
+  float I_xx;         /* mass * 2 * 1.5^2 / 12 */
+  float I_yy;         /* mass * (1.5^2 + 3^2) / 12 */
+  float wheel_radius; /* 0.32 m */
+  float c_g[3];       /* centre of gravity in the body frame: (2.981 / 2, 0, 0) */
+} mppib_racer_suspension_dyn_params;
+
 /* Elevation map of the RACER models (utils/texture_helpers/texture_helper.cuh:11-56 TextureParams + two_d_texture_helper.cu):
  * MPPIB_BLOB_ELEVATION_MAP = this header followed by width * height floats, row-major (value at row i, column j =
  * data[i * width + j]: TwoDTextureHelper's cpu_values_ layout). Clamp addressing, bilinear filtering, normalised
@@ -144,6 +161,9 @@ typedef struct mppib_elevation_map_header
   float resolution[3]; /* metres per cell */
   int use;
 } mppib_elevation_map_header;
+/* MPPIB_BLOB_NORMALS_MAP (TwoDTextureHelper<float4> map 0 of RacerDubinsElevationSuspension: normals_tex_helper_) is the
+ * same header followed by width * height float4 (x, y, z, w), row-major, queried with the same clamp + bilinear formula per
+ * channel. */
 
 /* QuadrotorDynamics (dynamics/quadrotor/quadrotor_dynamics.cuh:9-63). State POS(3) VEL(3) QUAT_W..Z(4) ANG_VEL(3);
  * controls ANG_RATE_X/Y/Z, THRUST. The default constructor's thrust range [0, 36] and zero_control[3] = GRAVITY

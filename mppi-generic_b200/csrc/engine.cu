@@ -112,12 +112,23 @@ static const PairEntry kPairs[] = {
   make_entry<plugins::QuadrotorDynamics, plugins::QuadrotorMapCost>(MPPIB_DYN_QUADROTOR, MPPIB_COST_QUADROTOR_MAP),
   make_entry<plugins::RacerDubinsElevationDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_DUBINS_ELEVATION,
                                                                                  MPPIB_COST_RACER_QUADRATIC),
+  make_entry<plugins::RacerSuspensionLSTMDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_SUSPENSION_LSTM,
+                                                                                MPPIB_COST_RACER_QUADRATIC),
 };
 
-// RacerDubinsElevationLSTMSteering with the steering LSTM on tensor cores (hidden_dim 32, head width <= 24)
+// RacerDubinsElevationLSTMSteering and RacerDubinsElevationSuspension with the steering LSTM on tensor cores (hidden_dim
+// 32, head width <= 24)
 static const PairEntry kPairsLstmMma[] = {
   make_entry<plugins::RacerLSTMMmaDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_LSTM, MPPIB_COST_RACER_QUADRATIC),
+  make_entry<plugins::RacerSuspensionLSTMMmaDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_SUSPENSION_LSTM,
+                                                                                   MPPIB_COST_RACER_QUADRATIC),
 };
+// the models whose steering is RacerDubinsElevationLSTMSteering's network: model_dims = { H, L1 }, weights in
+// MPPIB_BLOB_LSTM_WEIGHTS, one distribution
+static bool has_steering_lstm(int dyn_id)
+{
+  return dyn_id == MPPIB_DYN_RACER_LSTM || dyn_id == MPPIB_DYN_RACER_SUSPENSION_LSTM;
+}
 constexpr int kWsPspw8MaxRollouts = 6144;   // see mppib_create (warp-specialised Autorally K1)
 // the Autorally pair's default form, one entry per samples-per-warp width (chosen at create time from n_local)
 static const PairEntry kPairsMma[] = {
@@ -777,10 +788,10 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
   }
   // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
   // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network.
-  if (entry && desc.dynamics_id == MPPIB_DYN_RACER_LSTM && desc.model_dims[0] == lstm_mma::H &&
+  if (entry && has_steering_lstm(desc.dynamics_id) && desc.model_dims[0] == lstm_mma::H &&
       desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt)
     for (const auto& p : kPairsLstmMma)
-      if (p.cost_id == desc.cost_id)
+      if (p.dyn_id == desc.dynamics_id && p.cost_id == desc.cost_id)
         entry = &p;
   if (!entry)
     return fail(MPPIB_ERR_UNSUPPORTED, "no kernel registered for dynamics %d + cost %d", desc.dynamics_id, desc.cost_id);
@@ -1188,15 +1199,16 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
                 "ColoredNoise draws independent noise per distribution (colored_noise.cu:291); only "
                 "num_distributions == 1 is built");
 
-  if (desc->dynamics_id == MPPIB_DYN_RACER_LSTM)
+  if (has_steering_lstm(desc->dynamics_id))
   {
+    const char* model = desc->dynamics_id == MPPIB_DYN_RACER_LSTM ? "RacerDubinsElevationLSTMSteering" :
+                                                                     "RacerDubinsElevationSuspension";
     const int H = desc->model_dims[0], L1 = desc->model_dims[1];
     if (H < 1 || H > plugins::RacerLSTMDynamics::MAX_HIDDEN || L1 < 1 || L1 > plugins::RacerLSTMDynamics::MAX_HEAD)
-      return fail(MPPIB_ERR_INVALID_ARG, "RacerDubinsElevationLSTMSteering: model_dims = {hidden_dim %d, head width %d} "
-                                         "outside [1, %d] x [1, %d]",
+      return fail(MPPIB_ERR_INVALID_ARG, "%s: model_dims = {hidden_dim %d, head width %d} outside [1, %d] x [1, %d]", model,
                   H, L1, plugins::RacerLSTMDynamics::MAX_HIDDEN, plugins::RacerLSTMDynamics::MAX_HEAD);
     if (desc->num_distributions != 1)
-      return fail(MPPIB_ERR_UNSUPPORTED, "RacerDubinsElevationLSTMSteering is built for num_distributions == 1 only");
+      return fail(MPPIB_ERR_UNSUPPORTED, "%s is built for num_distributions == 1 only", model);
   }
   K1Overrides ov;
   const PairEntry* entry = nullptr;
@@ -1302,9 +1314,12 @@ bool ModelParams::uses(int which) const
     case MPPIB_BLOB_NN_WEIGHTS:
       return dyn_id_ == MPPIB_DYN_AUTORALLY_NN;
     case MPPIB_BLOB_LSTM_WEIGHTS:
-      return dyn_id_ == MPPIB_DYN_RACER_LSTM;
+      return has_steering_lstm(dyn_id_);
     case MPPIB_BLOB_ELEVATION_MAP:
-      return dyn_id_ == MPPIB_DYN_RACER_LSTM || dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION;
+      return dyn_id_ == MPPIB_DYN_RACER_LSTM || dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION ||
+             dyn_id_ == MPPIB_DYN_RACER_SUSPENSION_LSTM;
+    case MPPIB_BLOB_NORMALS_MAP:
+      return dyn_id_ == MPPIB_DYN_RACER_SUSPENSION_LSTM;
     case MPPIB_BLOB_COSTMAP:  // the costs whose blobs share the mppib_ar_standard_cost_params prefix
       return cost_id_ == MPPIB_COST_AR_STANDARD || cost_id_ == MPPIB_COST_AR_ROBUST;
     case MPPIB_BLOB_COST_TEXTURE:
@@ -1318,10 +1333,10 @@ bool ModelParams::uses(int which) const
 bool ModelParams::read_by_kernels(int which)
 {
   return which == MPPIB_BLOB_NN_WEIGHTS || which == MPPIB_BLOB_LSTM_WEIGHTS || which == MPPIB_BLOB_COSTMAP ||
-         which == MPPIB_BLOB_ELEVATION_MAP || which == MPPIB_BLOB_COST_TEXTURE;
+         which == MPPIB_BLOB_ELEVATION_MAP || which == MPPIB_BLOB_COST_TEXTURE || which == MPPIB_BLOB_NORMALS_MAP;
 }
 
-// the two maps are optional: without one the ground is flat, and the costmap term is 0
+// the maps are optional: without one the ground is flat, every normal points up, and the costmap term is 0
 int ModelParams::ready_for_solve() const
 {
   if (uses(MPPIB_BLOB_NN_WEIGHTS) && !is_set(MPPIB_BLOB_NN_WEIGHTS))
@@ -1360,9 +1375,10 @@ int ModelParams::upload_weights(Weights& w, int which, const char* what, const v
   return MPPIB_OK;
 }
 
-// A TwoDTextureHelper<float> map in the mppib_elevation_map_header + row-major floats format (params.h): validates the
-// header, grows the device buffer when needed and copies the values. `what` names the blob in the error text.
-int ModelParams::upload_map(Map& m, int which, const char* what, const void* host, size_t nbytes)
+// A TwoDTextureHelper<float> (channels 1) or <float4> (channels 4) map in the mppib_elevation_map_header + row-major
+// values format (params.h): validates the header, grows the device buffer when needed and copies the values. `what` names
+// the blob in the error text.
+int ModelParams::upload_map(Map& m, int which, const char* what, const void* host, size_t nbytes, int channels)
 {
   if (nbytes < sizeof(mppib_elevation_map_header))
     return fail(MPPIB_ERR_INVALID_ARG, "%s: %zu bytes is smaller than its header", what, nbytes);
@@ -1370,10 +1386,10 @@ int ModelParams::upload_map(Map& m, int which, const char* what, const void* hos
   memcpy(&h, host, sizeof(h));
   if (h.width < 2 || h.height < 2 || h.width > 16384 || h.height > 16384)
     return fail(MPPIB_ERR_INVALID_ARG, "%s: extent %d x %d (need 2 .. 16384 cells per side)", what, h.width, h.height);
-  const size_t cells = (size_t)h.width * h.height;
-  if (nbytes != sizeof(h) + cells * sizeof(float))
-    return fail(MPPIB_ERR_INVALID_ARG, "%s: got %zu bytes, expected %zu (header + %d x %d floats)", what, nbytes,
-                sizeof(h) + cells * sizeof(float), h.width, h.height);
+  const size_t cells = (size_t)h.width * h.height, floats = cells * channels;
+  if (nbytes != sizeof(h) + floats * sizeof(float))
+    return fail(MPPIB_ERR_INVALID_ARG, "%s: got %zu bytes, expected %zu (header + %d x %d x %d floats)", what, nbytes,
+                sizeof(h) + floats * sizeof(float), h.width, h.height, channels);
   for (int i = 0; i < 3; i++)
     if (!std::isfinite(h.origin[i]) || !std::isfinite(h.resolution[i]) || h.resolution[i] == 0.0f)
       return fail(MPPIB_ERR_INVALID_ARG, "%s: origin / resolution component %d is not usable", what, i);
@@ -1381,8 +1397,8 @@ int ModelParams::upload_map(Map& m, int which, const char* what, const void* hos
     if (!std::isfinite(h.rotations[i]))
       return fail(MPPIB_ERR_INVALID_ARG, "%s: rotation entry %d is not finite", what, i);
   set_ &= ~(1u << which);  // the device copy changes from here on
-  CUDA_TRY(m.d.reserve(cells, stream_));
-  CUDA_TRY(cudaMemcpyAsync(m.d, (const char*)host + sizeof(h), cells * sizeof(float), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(m.d.reserve(floats, stream_));
+  CUDA_TRY(cudaMemcpyAsync(m.d, (const char*)host + sizeof(h), floats * sizeof(float), cudaMemcpyHostToDevice, stream_));
   CUDA_TRY(cudaStreamSynchronize(stream_));
   m.hdr = h;
   return MPPIB_OK;
@@ -1434,6 +1450,15 @@ int ModelParams::set(int which, const void* host, size_t nbytes)
         return rc;
       elev_h_.assign(b, b + nbytes);
       break;
+    case MPPIB_BLOB_NORMALS_MAP:
+      // TwoDTextureHelper<float4> normals_tex_helper_ of RacerDubinsElevationSuspension (suspension_lstm.cu:18-57); NaN
+      // normals are the model's to handle (:291-294)
+      if (!uses(which))
+        return fail(MPPIB_ERR_INVALID_ARG, "normals map given to a dynamics without one");
+      if (int rc = upload_map(normals_, which, "normals map", host, nbytes, 4))
+        return rc;
+      normals_h_.assign(b, b + nbytes);
+      break;
     case MPPIB_BLOB_COST_TEXTURE:
       // QuadrotorMapCost's tex_helper_ map 0 (quadrotor_map_cost.cu:37-61), the same format
       if (!uses(which))
@@ -1480,6 +1505,14 @@ int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, flo
     const mppib_host_lstm net{ lstm_.h.data(), dims_[0], dims_[1], nullptr, nullptr,
                                is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr };
     return mppib_host_output_trajectory_lstm(dyn_.data(), &net, x0, u, T, dt, states, outputs);
+  }
+  if (dyn_id_ == MPPIB_DYN_RACER_SUSPENSION_LSTM)
+  {
+    const mppib_host_lstm net{ lstm_.h.data(), dims_[0], dims_[1], nullptr, nullptr,
+                               is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr };
+    return mppib_host_output_trajectory_racer_suspension(
+        dyn_.data(), &net, is_set(MPPIB_BLOB_NORMALS_MAP) ? (const mppib_elevation_map_header*)normals_h_.data() : nullptr,
+        x0, u, T, dt, states, outputs);
   }
   if (dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION)
     return mppib_host_output_trajectory_racer_dubins_elevation(

@@ -163,6 +163,15 @@ struct AuxFill<plugins::RacerLSTMDynamics::Aux>
   }
 };
 template <>
+struct AuxFill<plugins::RacerSuspensionParts::Aux>
+{
+  static void fill(plugins::RacerSuspensionParts::Aux& a, const ModelParams& m)
+  {
+    AuxFill<plugins::RacerLSTMDynamics::Aux>::fill(a, m);
+    a.normals = m.normals_map();
+  }
+};
+template <>
 struct AuxFill<plugins::RacerDubinsElevationDynamics::Aux>
 {
   static void fill(plugins::RacerDubinsElevationDynamics::Aux& a, const ModelParams& m)

@@ -1,13 +1,13 @@
 /*
  * model_params.cuh — the model a solve runs: every blob mppib_set_blob takes except the sampler's parameters (those are
  * NoiseSource's). The dynamics and cost parameter blobs are host copies that every launch copies into its kernel arguments;
- * the NN and LSTM weights, the costmap texture and the two maps (the RACER elevation map and QuadrotorMapCost's cost
- * texture, both in the mppib_elevation_map_header format) live in device memory. One member of mppib_engine; the
+ * the NN and LSTM weights, the costmap texture and the three maps (the RACER elevation map, the suspension model's
+ * normals map and QuadrotorMapCost's cost texture, all in the mppib_elevation_map_header format) live in device memory. One member of mppib_engine; the
  * definitions are in engine.cu.
  * - Which blobs a pair takes follows from its dynamics and cost ids, here only (uses()).
  * - A blob counts as set once its upload has succeeded; an upload that fails after its validation leaves it unset.
  * - Kernels read the device blobs (read_by_kernels()), so those may not change while a solve is in flight.
- * - A map that is not set reads as off (hdr.use == 0): flat ground, no costmap term.
+ * - A map that is not set reads as off (hdr.use == 0): flat ground, upright normals, no costmap term.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -40,6 +40,11 @@ public:
   cudaTextureObject_t costmap() const { return costmap_; }
   plugins::ElevationMap elevation_map() const { return view(elev_, MPPIB_BLOB_ELEVATION_MAP); }
   plugins::ElevationMap cost_texture() const { return view(cost_tex_, MPPIB_BLOB_COST_TEXTURE); }
+  plugins::NormalsMap normals_map() const
+  {
+    const plugins::ElevationMap v = view(normals_, MPPIB_BLOB_NORMALS_MAP);
+    return plugins::NormalsMap{ reinterpret_cast<const float4*>(v.data), v.hdr };
+  }
 
   // mppib_compute_control's roll-forward of one distribution through the library's host twins, with the host copies of
   // the blobs; the dynamics is a built-in one
@@ -53,12 +58,12 @@ private:
   };
   struct Map
   {
-    DeviceBuffer<float> d;  // width * height floats, row-major
+    DeviceBuffer<float> d;  // width * height values of `channels` floats each, row-major
     mppib_elevation_map_header hdr{};
   };
   bool uses(int which) const;
   int upload_weights(Weights& w, int which, const char* what, const void* host, size_t nbytes);
-  int upload_map(Map& m, int which, const char* what, const void* host, size_t nbytes);
+  int upload_map(Map& m, int which, const char* what, const void* host, size_t nbytes, int channels = 1);
   plugins::ElevationMap view(const Map& m, int which) const
   {
     plugins::ElevationMap v{ m.d, m.hdr };
@@ -74,8 +79,9 @@ private:
   unsigned set_ = 0;  // bit `which`: blob `which` is set
   std::vector<unsigned char> dyn_, cost_;
   Weights nn_, lstm_;
-  Map elev_, cost_tex_;
-  std::vector<unsigned char> elev_h_;  // the elevation map blob as set (header + floats), the host twins' format
+  Map elev_, cost_tex_, normals_;
+  // the elevation and normals map blobs as set (header + values), the host twins' format
+  std::vector<unsigned char> elev_h_, normals_h_;
   ArrayTexture costmap_;               // float4 array + its texture object
 };
 }  // namespace mppib

@@ -29,12 +29,14 @@ FLT_MAX = 3.4028234663852886e38
 # plugin ids (include/mppi_b200/params.h)
 DYN_CARTPOLE, DYN_DOUBLE_INTEGRATOR, DYN_AUTORALLY_NN, DYN_RACER_LSTM, DYN_QUADROTOR = 0, 1, 2, 3, 4
 DYN_RACER_DUBINS_ELEVATION = 5
+DYN_RACER_SUSPENSION_LSTM = 6
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
 COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
 COST_QUADROTOR_MAP = 7
 SAMPLER_GAUSSIAN, SAMPLER_COLORED_NOISE, SAMPLER_NLN = 0, 1, 2
 BLOB_DYN, BLOB_COST, BLOB_SAMPLER, BLOB_NN_WEIGHTS, BLOB_COSTMAP, BLOB_LSTM_WEIGHTS, BLOB_ELEVATION_MAP = range(7)
 BLOB_COST_TEXTURE = 7
+BLOB_NORMALS_MAP = 8
 # QuadrotorMapCost's terms (host_twins.h: mppib_quadrotor_map_term)
 QMAP_GATE_SIDE, QMAP_HEADING, QMAP_HEIGHT, QMAP_SPEED, QMAP_STABILIZING, QMAP_WAYPOINT = range(6)
 FLAG_WRITEBACK_CONTROLS, FLAG_NO_TMA, FLAG_CURAND_HOST_API, FLAG_NO_PREFETCH, FLAG_NN_TENSOR, FLAG_RMPPI = 1, 2, 4, 8, 16, 32
@@ -160,6 +162,14 @@ class RacerLSTMDynParams(C.Structure):
                 ("Q_omega_v", C.c_float), ("Q_omega_steering", C.c_float)]
 
 
+class RacerSuspensionDynParams(C.Structure):
+    """mppib_racer_suspension_dyn_params (params.h): the LSTM model's fields, then RacerDubinsElevationSuspensionParams' own
+    (racer_dubins_elevation_suspension_lstm.cuh:54-63); c_g is the centre of gravity in the body frame."""
+    _fields_ = RacerLSTMDynParams._fields_ + [("spring_k", C.c_float), ("drag_c", C.c_float), ("mass", C.c_float),
+                                              ("I_xx", C.c_float), ("I_yy", C.c_float), ("wheel_radius", C.c_float),
+                                              ("c_g", C.c_float * 3)]
+
+
 class RacerQuadraticCostParams(C.Structure):
     _fields_ = [("control_cost_coeff", C.c_float * MAX_C), ("discount", C.c_float), ("desired_speed", C.c_float),
                 ("speed_coeff", C.c_float), ("desired_yaw", C.c_float), ("yaw_coeff", C.c_float),
@@ -256,6 +266,28 @@ class TwoDTextureHelper:
         return float(L.mppib_host_elevation_at_world_pose(b.ctypes.data, float(point[0]), float(point[1]), float(point[2])))
 
 
+class TwoDTextureHelperFloat4(TwoDTextureHelper):
+    """TwoDTextureHelper<float4> for ONE map (RacerDubinsElevationSuspension's normals_tex_helper_): the same methods, values
+    [height][width][4]; blob() travels as MPPIB_BLOB_NORMALS_MAP and queryTextureAtWorldPose returns the four channels."""
+
+    def updateTexture(self, index: int, values, column_major: bool = False) -> None:
+        v = _f32(values).reshape(-1, 4)
+        w, h = self.hdr.width, self.hdr.height
+        if v.shape[0] != w * h:
+            raise ValueError(f"invalid size to updateTexture {v.shape[0]} != {w * h}")  # two_d_texture_helper.cu:27-32
+        self.values = (v.reshape(w, h, 4).transpose(1, 0, 2) if column_major else v.reshape(h, w, 4)).copy()
+        self._blob = None
+
+    def queryTextureAtWorldPose(self, index: int, point) -> np.ndarray:
+        b = self.blob()
+        out = np.zeros(4, np.float32)
+        L = lib()
+        L.mppib_host_normals_at_world_pose.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p]
+        L.mppib_host_normals_at_world_pose(b.ctypes.data, float(point[0]), float(point[1]), float(point[2]),
+                                           out.ctypes.data)
+        return out
+
+
 class CartpoleCostParams(C.Structure):
     _fields_ = [("control_cost_coeff", C.c_float * MAX_C), ("discount", C.c_float),
                 ("cart_position_coeff", C.c_float), ("cart_velocity_coeff", C.c_float),
@@ -319,7 +351,8 @@ ABI_SYMBOLS = [
     "mppib_host_slide_controls", "mppib_host_output_trajectory", "mppib_host_free_energy",
     "mppib_host_merge_records", "mppib_host_step_lstm", "mppib_host_output_trajectory_lstm",
     "mppib_host_step_racer_dubins_elevation", "mppib_host_output_trajectory_racer_dubins_elevation",
-    "mppib_host_grad_racer_dubins_elevation",
+    "mppib_host_grad_racer_dubins_elevation", "mppib_host_step_racer_suspension",
+    "mppib_host_output_trajectory_racer_suspension", "mppib_host_normals_at_world_pose",
     "mppib_host_elevation_at_world_pose", "mppib_host_static_settling", "mppib_host_lstm_initialize",
     "mppib_set_rmppi", "mppib_init_eval", "mppib_set_tsallis", "mppib_sample_trajectories", "mppib_nominal_trajectory", "mppib_compute_control", "mppib_host_npz_read", "mppib_comm_p2p_handle", "mppib_comm_p2p_open", "mppib_host_rmppi_line_search_weights", "mppib_host_rmppi_candidates",
     "mppib_host_rmppi_best_index", "mppib_set_ddp", "mppib_ddp_feedback",
@@ -391,6 +424,9 @@ def lib() -> C.CDLL:
     L.mppib_host_step_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, C.c_float, vp, vp, vp]
     L.mppib_host_output_trajectory_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, C.c_int, C.c_float, vp, vp]
     L.mppib_host_grad_racer_dubins_elevation.argtypes = [vp, vp, vp, vp, vp]
+    L.mppib_host_step_racer_suspension.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, vp, C.c_float, vp, vp, vp]
+    L.mppib_host_output_trajectory_racer_suspension.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, vp, C.c_int, C.c_float,
+                                                                 vp, vp]
     L.mppib_set_rmppi.argtypes = [vp, C.c_float, vp]
     L.mppib_set_tsallis.argtypes = [vp, C.c_float, C.c_float]
     L.mppib_init_eval.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]
@@ -581,6 +617,14 @@ class NeuralNetModel(_Dynamics):
             chunks += [W_.ravel(), b.ravel()]
             i += 1
         self.updateModel(layers, np.concatenate(chunks))
+
+
+def _npz_has(path: str, name: str) -> bool:
+    try:
+        npz_read(path, name)
+        return True
+    except MppibError:
+        return False
 
 
 def npz_read(path: str, name: str) -> np.ndarray:
@@ -914,6 +958,126 @@ class RacerDubinsElevationLSTMSteering(RacerDubinsElevation):
         net = self._host_net(h, c)
         _check(lib().mppib_host_output_trajectory_lstm(C.byref(self.params), C.byref(net), _ptr(_f32(x0)), _ptr(u), T,
                                                        C.c_float(dt), _ptr(states), _ptr(outputs)))
+
+
+class RacerDubinsElevationSuspension(RacerDubinsElevationLSTMSteering):
+    """dynamics/racer_dubins/racer_dubins_elevation_suspension_lstm.cuh — RacerDubinsElevationSuspension(init_input_dim,
+    init_hidden_dim, init_output_layers, input_dim, hidden_dim, output_layers, init_len) / RacerDubinsElevationSuspension(path):
+    the LSTM-steering vehicle (S24 C2 O28) whose roll, pitch and heave are integrated from four spring-damper wheels over the
+    elevation map (``getTextureHelper()``) and the normals map (``getTextureHelperNormals()``). The network, its weights
+    and model_dims are the LSTM model's. One distribution only, like the LSTM model."""
+    DYN_ID, STATE_DIM, CONTROL_DIM, OUTPUT_DIM = DYN_RACER_SUSPENSION_LSTM, 24, 2, 28
+    # racer_dubins_elevation_suspension_lstm.cuh:25-52
+    (VEL_X, YAW, POS_X, POS_Y, STEER_ANGLE, BRAKE_STATE, ROLL, PITCH, CG_POS_Z, CG_VEL_I_Z, ROLL_RATE, PITCH_RATE,
+     STEER_ANGLE_RATE) = range(13)
+    UNCERTAINTY_POS_X = 13  # ... the ten entries to 22, then FILLER_1
+
+    def __init__(self, init_input_dim=3, init_hidden_dim: int = 20, init_output_layers: Sequence[int] = (23, 100, 8),
+                 input_dim: int = 4, hidden_dim: int = 4, output_layers: Sequence[int] = (8, 20, 1), init_len: int = 11):
+        path = init_input_dim if isinstance(init_input_dim, str) else None
+        if path:  # the architecture as the file's arrays give it (LSTMLSTMHelper(path), lstm_lstm_helper.cu:14-31)
+            pre = "model/" if _npz_has(path, "model/lstm/weight_hh_l0") else ""
+            H = npz_read(path, pre + "lstm/weight_hh_l0").shape[1]
+            L1 = npz_read(path, pre + "output/dynamics_W1").shape[0]
+            init_input_dim, init_hidden_dim, init_output_layers = 3, 20, (23, 100, 2 * H)
+            input_dim, hidden_dim, output_layers, init_len = 4, H, (H + 4, L1, 1), 11
+        super().__init__(init_input_dim, init_hidden_dim, init_output_layers, input_dim, hidden_dim, output_layers,
+                         init_len)
+        base = self.params
+        p = RacerSuspensionDynParams()
+        C.memmove(C.byref(p), C.byref(base), C.sizeof(RacerLSTMDynParams))
+        # racer_dubins_elevation_suspension_lstm.cuh:54-63
+        p.spring_k, p.drag_c, p.mass = 14000.0, 1000.0, 1447.0
+        m32 = np.float32(1447.0)
+        p.I_xx = float(np.float32(np.float32(np.float32(np.float32(1.0) / np.float32(12)) * m32) * np.float32(2)) *
+                       np.float32(2.25))
+        p.I_yy = float(np.float32(np.float32(np.float32(1.0) / np.float32(12)) * m32) * np.float32(2.25 + 9.0))
+        p.wheel_radius = 0.32
+        p.c_g[0], p.c_g[1], p.c_g[2] = float(np.float32(2.981) * np.float32(0.5)), 0.0, 0.0
+        self.params = p
+        self.normals_tex_helper_ = TwoDTextureHelperFloat4()
+        if path:
+            self.loadParamsLSTM(path)
+
+    def getParams(self) -> RacerSuspensionDynParams:
+        out = RacerSuspensionDynParams()
+        C.memmove(C.byref(out), C.byref(self.params), C.sizeof(RacerSuspensionDynParams))
+        return out
+
+    def setParams(self, params: RacerSuspensionDynParams) -> None:
+        C.memmove(C.byref(self.params), C.byref(params), C.sizeof(RacerSuspensionDynParams))
+
+    def getTextureHelperNormals(self) -> "TwoDTextureHelperFloat4":
+        return self.normals_tex_helper_
+
+    def updateRotation(self, rotation) -> None:
+        """Both maps take the same rotation (racer_dubins_elevation_suspension_lstm.cuh:133-137)."""
+        self.tex_helper_.updateRotation(0, rotation)
+        self.normals_tex_helper_.updateRotation(0, rotation)
+
+    def setNormalsMap(self, normals, resolution, origin=(0.0, 0.0, 0.0), rotation=None, enable: bool = True) -> None:
+        """Convenience over the normals helper: normals [height][width][3 or 4] (w = 0 when three are given)."""
+        v = _f32(normals)
+        if v.shape[-1] == 3:
+            v = np.concatenate([v, np.zeros(v.shape[:-1] + (1,), np.float32)], axis=-1)
+        t = self.normals_tex_helper_
+        t.setExtent(0, v.shape[1], v.shape[0])
+        t.updateTexture(0, v)
+        t.updateResolution(0, resolution)
+        t.updateOrigin(0, origin)
+        if rotation is not None:
+            t.updateRotation(0, rotation)
+        t.enableTexture(0) if enable else t.disableTexture(0)
+
+    def stateFromMap(self, m: dict) -> np.ndarray:
+        """racer_dubins_elevation_suspension_lstm.cu:527-611: CG_POS_Z is the z of the centre of gravity in the world frame,
+        CG_VEL_I_Z the base link's inertial vertical speed less OMEGA_Y * c_g.x; the uncertainty diagonal gets a 1e-6
+        floor. A missing key gives an all-NaN state."""
+        keys = ("VEL_X", "VEL_Z", "POS_X", "POS_Y", "POS_Z", "OMEGA_X", "OMEGA_Y", "ROLL", "PITCH", "YAW", "STEER_ANGLE",
+                "STEER_ANGLE_RATE", "BRAKE_STATE")
+        if any(k not in m for k in keys):
+            return np.full(24, np.nan, np.float32)
+        f = np.float32
+        s = np.zeros(24, np.float32)
+        g = [f(self.params.c_g[i]) for i in range(3)]
+        s[self.POS_X], s[self.POS_Y], s[self.VEL_X] = m["POS_X"], m["POS_Y"], m["VEL_X"]
+        pitch = f(m["PITCH"])
+        bl_v_I_z = f(f(f(m["VEL_Z"]) * f(math.cos(pitch))) - f(f(m["VEL_X"]) * f(math.sin(pitch))))
+        s[self.CG_VEL_I_Z] = bl_v_I_z - f(m["OMEGA_Y"]) * g[0]
+        s[self.STEER_ANGLE], s[self.STEER_ANGLE_RATE] = m["STEER_ANGLE"], m["STEER_ANGLE_RATE"]
+        s[self.ROLL], s[self.PITCH], s[self.YAW] = m["ROLL"], m["PITCH"], m["YAW"]
+        # bodyOffsetToWorldPoseEuler(c_g, (x, y, POS_Z), (roll, pitch, yaw)): the z row of Euler2DCM_NWU (host branch)
+        sr, cr = f(math.sin(f(m["ROLL"]))), f(math.cos(f(m["ROLL"])))
+        sp, cp = f(math.sin(pitch)), f(math.cos(pitch))
+        s[self.CG_POS_Z] = f(f(f(-sp * g[0]) + f(sr * cp) * g[1]) + f(cr * cp) * g[2]) + f(m["POS_Z"])
+        s[self.ROLL_RATE], s[self.PITCH_RATE], s[self.BRAKE_STATE] = m["OMEGA_X"], m["OMEGA_Y"], m["BRAKE_STATE"]
+        for i in range(4):
+            s[self.UNCERTAINTY_POS_X + i] = max(s[self.UNCERTAINTY_POS_X + i], f(1e-6))
+        return s
+
+    def _normals_ptr(self):
+        b = self.normals_tex_helper_.blob()
+        return None if b is None else b.ctypes.data
+
+    def step(self, state, control, dt: float, hidden=None, cell=None):
+        """Host step (racer_dubins_elevation_suspension_lstm.cu:168-197); returns (next_state, state_der, output, hidden,
+        cell)."""
+        h0, c0 = self.initial_hidden_cell()
+        h = h0 if hidden is None else _f32(hidden).copy()
+        c = c0 if cell is None else _f32(cell).copy()
+        x, u = _f32(state), _f32(control)
+        xn, xd, y = np.zeros(24, np.float32), np.zeros(24, np.float32), np.zeros(28, np.float32)
+        net = self._host_net(h, c)
+        _check(lib().mppib_host_step_racer_suspension(C.addressof(self.params), C.byref(net), self._normals_ptr(), _ptr(x),
+                                                      _ptr(u), C.c_float(dt), _ptr(xn), _ptr(xd), _ptr(y)))
+        return xn, xd, y, h, c
+
+    def output_trajectory(self, x0, u, T: int, dt: float, states: np.ndarray, outputs: np.ndarray) -> None:
+        h, c = self.initial_hidden_cell()
+        net = self._host_net(h, c)
+        _check(lib().mppib_host_output_trajectory_racer_suspension(C.addressof(self.params), C.byref(net),
+                                                                   self._normals_ptr(), _ptr(_f32(x0)), _ptr(_f32(u)), T,
+                                                                   C.c_float(dt), _ptr(states), _ptr(outputs)))
 
 
 class _Cost:
@@ -1364,13 +1528,17 @@ class Engine:
         if self.dyn.DYN_ID == DYN_AUTORALLY_NN:
             w = _f32(self.dyn.nn_theta)
             _check(L.mppib_set_blob(self._h, BLOB_NN_WEIGHTS, _ptr(w), w.nbytes))
-        if self.dyn.DYN_ID == DYN_RACER_LSTM:
+        if self.dyn.DYN_ID in (DYN_RACER_LSTM, DYN_RACER_SUSPENSION_LSTM):
             w = _f32(self.dyn.lstm_theta)
             _check(L.mppib_set_blob(self._h, BLOB_LSTM_WEIGHTS, _ptr(w), w.nbytes))
-        if self.dyn.DYN_ID in (DYN_RACER_LSTM, DYN_RACER_DUBINS_ELEVATION):
+        if self.dyn.DYN_ID in (DYN_RACER_LSTM, DYN_RACER_DUBINS_ELEVATION, DYN_RACER_SUSPENSION_LSTM):
             m = self.dyn.tex_helper_.blob()
             if m is not None:  # TwoDTextureHelper::copyToDevice
                 _check(L.mppib_set_blob(self._h, BLOB_ELEVATION_MAP, m.ctypes.data, m.nbytes))
+        if self.dyn.DYN_ID == DYN_RACER_SUSPENSION_LSTM:
+            m = self.dyn.normals_tex_helper_.blob()
+            if m is not None:
+                _check(L.mppib_set_blob(self._h, BLOB_NORMALS_MAP, m.ctypes.data, m.nbytes))
         if self.cost.COST_ID in (COST_AR_STANDARD, COST_AR_ROBUST):
             if self.cost.costmap is None:
                 raise MppibError(-9, f"{type(self.cost).__name__} has no costmap (call loadTrackData / setCostmap)")

@@ -260,6 +260,64 @@ def racer_elevation_tube(N: int = 8192, T: int = 100, use_map: bool = True) -> W
     return w
 
 
+def racer_hill_maps(seed: int = 13, resolution: float = 0.5) -> tuple:
+    """(elevation, normals) helpers for the suspension model: x in [-10, 90], y in [-30, 30] m, twelve seeded Gaussian hills
+    (heights 0.2 .. 0.8 m, widths 3 .. 8 m); the normals are (-dz/dx, -dz/dy, 1) normalised, from the heights' central
+    differences."""
+    xb, yb = (-10.0, 90.0), (-30.0, 30.0)
+    w, h = int(round((xb[1] - xb[0]) / resolution)), int(round((yb[1] - yb[0]) / resolution))
+    cx = xb[0] + (np.arange(w) + 0.5) * resolution
+    cy = yb[0] + (np.arange(h) + 0.5) * resolution
+    X, Y = np.meshgrid(cx, cy)  # [h][w]
+    rng = np.random.RandomState(seed)
+    z = np.zeros_like(X)
+    for _ in range(12):
+        x0, y0 = rng.uniform(*xb), rng.uniform(*yb)
+        z += rng.uniform(0.2, 0.8) * np.exp(-((X - x0) ** 2 + (Y - y0) ** 2) / (2 * rng.uniform(3.0, 8.0) ** 2))
+    dzdy, dzdx = np.gradient(z, resolution)
+    n = np.stack([-dzdx, -dzdy, np.ones_like(z)], axis=-1)
+    n /= np.linalg.norm(n, axis=-1, keepdims=True)
+    elev = H.TwoDTextureHelper()
+    elev.setExtent(0, w, h)
+    elev.updateTexture(0, z.astype(np.float32))
+    elev.updateOrigin(0, (xb[0], yb[0], 0.0))
+    elev.updateResolution(0, resolution)
+    elev.enableTexture(0)
+    normals = H.TwoDTextureHelperFloat4()
+    normals.setExtent(0, w, h)
+    normals.updateTexture(0, np.concatenate([n, np.zeros(z.shape + (1,))], axis=-1).astype(np.float32))
+    normals.updateOrigin(0, (xb[0], yb[0], 0.0))
+    normals.updateResolution(0, resolution)
+    normals.enableTexture(0)
+    return elev, normals
+
+
+def racer_suspension(N: int = 65536, T: int = 150, hidden_dim: int = 4, use_maps: bool = True, head_hidden: int = 20,
+                     colored: bool = True) -> Workload:
+    """RacerDubinsElevationSuspension at C5's settings (racer_lstm(): the same network, weights, sampler and cost) over
+    racer_hill_maps(), or flat ground with upright normals when use_maps is False. The car starts at 3 m/s with its centre
+    of gravity one wheel radius above the ground under it."""
+    dyn = H.RacerDubinsElevationSuspension(3, 20, (23, 100, 2 * hidden_dim), 4, hidden_dim, (hidden_dim + 4, head_hidden, 1),
+                                           11)
+    dyn.setControlRanges([(-1.0, 1.0), (-1.0, 1.0)])
+    dyn.setAllValues(*synthetic_lstm_weights(hidden_dim, head_hidden, 2))
+    x0 = np.zeros((1, 24), np.float32)
+    x0[0, dyn.VEL_X] = 3.0
+    x0[0, dyn.UNCERTAINTY_POS_X:dyn.UNCERTAINTY_POS_X + 4] = 1e-6
+    ground = 0.0
+    if use_maps:
+        dyn.tex_helper_, dyn.normals_tex_helper_ = racer_hill_maps()
+        ground = dyn.tex_helper_.queryTextureAtWorldPose(0, (dyn.params.c_g[0], 0.0, 0.0))
+    x0[0, dyn.CG_POS_Z] = ground + dyn.params.wheel_radius
+    cost = H.RacerQuadraticCost()
+    cost.params.desired_speed = 1.2
+    sampler = H.ColoredNoiseDistribution(2, [0.3, 0.3], [1.0, 1.0]) if colored else H.GaussianDistribution(2, [0.3, 0.3])
+    U0 = np.zeros((1, T, 2), np.float32)
+    tag = ("maps" if use_maps else "flat") + ("" if colored else "_gaussian")
+    return Workload(f"racer_suspension_H{hidden_dim}_{tag}_N{N}_T{T}", "vanilla", dyn, cost, sampler, N, T, 1, 0.02, 1.0,
+                    0.0, x0, U0)
+
+
 def quadrotor(N: int = 8192, T: int = 100) -> Workload:
     """Quadrotor + quadratic cost, VanillaMPPI (instantiations/quadrotor_mppi/quadrotor_mppi.cuh): fly from the origin
     to a goal 4 m away and 2 m up, hovering there. The only CONTROL_DIM = 4 pair (one 16-byte noise group per step)."""
