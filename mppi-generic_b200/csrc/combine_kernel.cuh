@@ -9,7 +9,8 @@
  * K1 already produced, per block b, (beta_b, eta_b, sum w^2_b, V_b[t][c] = sum_n w_n u_n) against its LOCAL baseline.
  * With beta = min_b beta_b and s_b = expf(-(beta_b - beta)/lambda):
  *     eta = sum_b s_b eta_b,   sum w^2 = sum_b s_b^2 w2_b,   U = (sum_b s_b V_b) / eta
- * which is algebraically the reference's two-pass formula (w_n = expf(-(c_n-beta_b)/lambda) * s_b). The same kernel
+ * which is algebraically the reference's two-pass formula (w_n = expf(-(c_n-beta_b)/lambda) * s_b). A record whose
+ * baseline is +inf (every cost +inf) is empty, s_b = 0 (softmin.h). The same kernel
  * merges the per-GPU records after the NCCL all-gather (records = ranks, normalize = 1).
  *
  * Launch: grid (ceil(TC/32), D), block 512 = 16 warps x 32 columns; block-wide warp-shuffle reductions, the rescale
@@ -80,7 +81,7 @@ __global__ void __launch_bounds__(kCombineCols* kCombineGroups)
     const int b = tid + i * (int)blockDim.x;
     if (b < nrec)
     {
-      const float s = expf(-lambda_inv * (h[i].x - beta));
+      const float s = softmin_weight(h[i].x, beta, lambda_inv);  // 0 for an empty record (baseline +inf)
       scale_sh[b] = s;
       eta += (double)s * (double)h[i].y;
       w2 += (double)s * (double)s * (double)h[i].z;
@@ -224,7 +225,7 @@ __global__ void __launch_bounds__(512)
     for (int r = 0; r < world; r++)
     {
       const float* h = g + (size_t)r * rec + d * pstride;
-      const float s = expf(-lambda_inv * (h[0] - beta));
+      const float s = softmin_weight(h[0], beta, lambda_inv);  // 0 for an empty record (baseline +inf)
       scale_sh[d][r] = s;
       eta += (double)s * (double)h[1];
       w2 += (double)s * (double)s * (double)h[2];

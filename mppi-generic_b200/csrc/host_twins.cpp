@@ -18,6 +18,7 @@
 
 #include "../../include/mppi_b200.h"
 #include "../../include/mppi_b200/host_twins.h"
+#include "softmin.h"
 
 namespace
 {
@@ -1545,7 +1546,7 @@ int mppib_host_merge_records(const float* records, int nrec, int D, int TC, int 
     for (int b = 0; b < nrec; b++)
     {
       const float* r = rec + b * rstride;
-      const float s = expf(-lambda_inv * (r[0] - beta));
+      const float s = mppib::softmin_weight(r[0], beta, lambda_inv);  // 0 for an empty record (baseline +inf)
       eta += (double)s * (double)r[1];
       w2 += (double)s * (double)s * (double)r[2];
       for (int c = 0; c < TC; c++)

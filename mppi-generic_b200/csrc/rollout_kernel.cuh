@@ -551,7 +551,7 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
 #pragma unroll
     for (int sp = 0; sp < SPT; sp++)
     {
-      const float w = valid[sp] ? expf(-args.lambda_inv * (cost[sp * D + d] - beta_b)) : 0.0f;
+      const float w = valid[sp] ? softmin_weight(cost[sp * D + d], beta_b, args.lambda_inv) : 0.0f;
       if (owner)
         w_s[d * bx + row[sp]] = w;
       wsum += w;

@@ -459,7 +459,7 @@ __global__ void __launch_bounds__(nn_tc::kRows, 2)
     float beta_b = scratch[0];
     for (int i = 1; i < 4; i++)
       beta_b = fminf(beta_b, scratch[i]);
-    const float w = valid ? expf(-args.lambda_inv * (cost - beta_b)) : 0.0f;
+    const float w = valid ? softmin_weight(cost, beta_b, args.lambda_inv) : 0.0f;
     w_s[tid] = w;
     const float sw = warp_sum(w), sw2 = warp_sum(w * w);
     if (lane == 0)
