@@ -371,6 +371,58 @@ public:
 
 typedef Matrix<float, 3, 3> Matrix3f;
 typedef Matrix<float, 3, 1> Vector3f;
+
+// unit quaternion (w, x, y, z) with the accessors, conjugate, rotation matrix and vector rotation the host layer uses
+class Quaternionf
+{
+public:
+  Quaternionf() : w_(1.0f), x_(0.0f), y_(0.0f), z_(0.0f)
+  {
+  }
+  Quaternionf(float w, float x, float y, float z) : w_(w), x_(x), y_(y), z_(z)
+  {
+  }
+  float w() const
+  {
+    return w_;
+  }
+  float x() const
+  {
+    return x_;
+  }
+  float y() const
+  {
+    return y_;
+  }
+  float z() const
+  {
+    return z_;
+  }
+  Quaternionf conjugate() const
+  {
+    return Quaternionf(w_, -x_, -y_, -z_);
+  }
+  Matrix3f toRotationMatrix() const
+  {  // Eigen's formula
+    const float tx = 2 * x_, ty = 2 * y_, tz = 2 * z_, twx = tx * w_, twy = ty * w_, twz = tz * w_, txx = tx * x_,
+                txy = ty * x_, txz = tz * x_, tyy = ty * y_, tyz = tz * y_, tzz = tz * z_;
+    Matrix3f m;
+    m << 1 - (tyy + tzz), txy - twz, txz + twy, txy + twz, 1 - (txx + tzz), tyz - twx, txz - twy, tyz + twx,
+        1 - (txx + tyy);
+    return m;
+  }
+  Vector3f operator*(const Vector3f& v) const
+  {
+    const Matrix3f m = toRotationMatrix();
+    Vector3f r;
+    for (int i = 0; i < 3; i++)
+      r(i) = m(i, 0) * v(0) + m(i, 1) * v(1) + m(i, 2) * v(2);
+    return r;
+  }
+
+private:
+  float w_, x_, y_, z_;
+};
 }  // namespace Eigen
 #else
 #include <Eigen/Dense>

@@ -8,6 +8,7 @@
  *   mppib_host_output_trajectory    Controller::computeOutputTrajectoryHelper   controller.cuh:643-663
  *   mppib_host_step_lstm / mppib_host_output_trajectory_lstm   the same two for RacerDubinsElevationLSTMSteering
  *   mppib_host_step_racer_suspension / mppib_host_output_trajectory_racer_suspension   ... for RacerDubinsElevationSuspension
+ *   mppib_host_step_racer_rigid_suspension / _output_trajectory_racer_rigid_suspension ... for RacerSuspension (rigid body)
  *   mppib_host_free_energy          mppi::kernels::computeFreeEnergy      include/mppi/core/mppi_common.cu:1065-1081
  *   mppib_host_merge_records        (no reference counterpart: the log-sum-exp merge of rollout shards, SURVEY §8e)
  *   mppib_host_state_cost           the robust costs' and QuadrotorMapCost's host computeStateCost and terms (below)
@@ -72,6 +73,17 @@ int mppib_host_step_racer_suspension(const void* dyn_params, const mppib_host_ls
 int mppib_host_output_trajectory_racer_suspension(const void* dyn_params, const mppib_host_lstm* net,
                                                   const mppib_elevation_map_header* normals, const float* x0,
                                                   const float* u, int T, float dt, float* states, float* outputs);
+/* RacerSuspension, the rigid body (dynamics/racer_suspension/racer_suspension.cu; blob mppib_racer_rigid_suspension_dyn_params,
+ * S = 14, O = 26). _state_deriv: the host computeStateDeriv (:93-298) on the plane z = 0, outputs of x, and when
+ * omega_jacobian != NULL the 3x3 omegaJacobian row-major, as written (f_r_B_i_Jac = f_r_C_i_Jac, :215). _step: the host
+ * step (:31-45), the body rates by approximate implicit Euler through that Jacobian, then q / |q|; y = the outputs of x.
+ * The device step is explicit Euler on every state (DESIGN §8). */
+int mppib_host_state_deriv_racer_rigid_suspension(const void* dyn_params, const float* x, const float* u, float* xdot,
+                                                  float* y, float* omega_jacobian);
+int mppib_host_step_racer_rigid_suspension(const void* dyn_params, const float* x, const float* u, float dt, float* x_next,
+                                           float* xdot, float* y);
+int mppib_host_output_trajectory_racer_rigid_suspension(const void* dyn_params, const float* x0, const float* u, int T,
+                                                        float dt, float* states, float* outputs);
 /* TwoDTextureHelper<float4>::queryTextureAtWorldPose on the host: out4 = the four channels, each by the float map's
  * formula (mppib_host_elevation_at_world_pose); map NULL: (0, 0, 1, 0). */
 void mppib_host_normals_at_world_pose(const mppib_elevation_map_header* map, float x, float y, float z, float* out4);

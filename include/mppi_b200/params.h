@@ -27,6 +27,7 @@ enum mppib_dynamics_id
   MPPIB_DYN_QUADROTOR = 4,         /* dynamics/quadrotor/quadrotor_dynamics.cuh          S13 C4 O13 */
   MPPIB_DYN_RACER_DUBINS_ELEVATION = 5, /* dynamics/racer_dubins/racer_dubins_elevation.cuh  S19 C2 O28 */
   MPPIB_DYN_RACER_SUSPENSION_LSTM = 6,  /* dynamics/racer_dubins/racer_dubins_elevation_suspension_lstm.cuh S24 C2 O28 */
+  MPPIB_DYN_RACER_SUSPENSION = 7,       /* dynamics/racer_suspension/racer_suspension.cuh (rigid body)  S14 C2 O26 */
   MPPIB_DYN_COUNT
 };
 
@@ -147,6 +148,36 @@ typedef struct mppib_racer_suspension_dyn_params
   float wheel_radius; /* 0.32 m */
   float c_g[3];       /* centre of gravity in the body frame: (2.981 / 2, 0, 0) */
 } mppib_racer_suspension_dyn_params;
+
+/* RacerSuspension (dynamics/racer_suspension/racer_suspension.cuh:8-128, RacerSuspensionParams), the 6-DoF rigid body on
+ * four spring-damper wheels, field for field: float3 as three floats, the fields recalcParams() derives included (the host
+ * classes derive them; the engine reads them as given). Not to be confused with id 6's mppib_racer_suspension_dyn_params.
+ * Wheels in the order front left, front right, rear left, rear right. No map: the model's ground is the plane z = 0. */
+typedef struct mppib_racer_rigid_suspension_dyn_params
+{
+  mppib_control_limits lim;
+  float wheel_radius;                  /* 0.32 m */
+  float mass;                          /* 1447 kg */
+  float wheel_base;                    /* 2.981 m */
+  float width;                         /* 1.5 m */
+  float height;                        /* 1.5 m */
+  float gravity;                       /* -9.81 */
+  float k_s[4];                        /* 14000 N / m */
+  float c_s[4];                        /* 2000 N s / m */
+  float l_0[4];                        /* derived: wheel_radius + mass / 4 * (-gravity) / k_s[i] */
+  float cg_pos_wrt_base_link[3];       /* derived: (wheel_base / 2, 0, 0.2) */
+  float wheel_pos_wrt_base_link[4][3]; /* derived: (wheel_base, +-width / 2, 0), (0, +-width / 2, 0) */
+  float Jxx, Jyy, Jzz;                 /* derived, in double: mass / 12 * (sum of two squared extents) */
+  float mu;                            /* 0.65 */
+  float v_slip;                        /* 0.1 m / s */
+  float c_t;                           /* 3.0 */
+  float c_b;                           /* 10.0 */
+  float c_v;                           /* 0.2 */
+  float c_0;                           /* 0 */
+  float steering_constant;             /* 0.6 */
+  float steer_command_angle_scale;     /* -2.45 */
+  int gear_sign;                       /* 1 (not read by the model) */
+} mppib_racer_rigid_suspension_dyn_params;
 
 /* Elevation map of the RACER models (utils/texture_helpers/texture_helper.cuh:11-56 TextureParams + two_d_texture_helper.cu):
  * MPPIB_BLOB_ELEVATION_MAP = this header followed by width * height floats, row-major (value at row i, column j =
@@ -279,6 +310,12 @@ MPPIB_AR_PREFIX_SAME(map_height)
 static_assert(offsetof(mppib_ar_robust_cost_params, heading_coeff) == sizeof(mppib_ar_standard_cost_params),
               "heading_coeff follows the standard prefix");
 #undef MPPIB_AR_PREFIX_SAME
+/* the rigid-body RACER blob: 16 limit floats, then 45 four-byte fields in RacerSuspensionParams' order */
+static_assert(offsetof(mppib_racer_rigid_suspension_dyn_params, wheel_radius) == 64, "limits first");
+static_assert(offsetof(mppib_racer_rigid_suspension_dyn_params, l_0) == 64 + 14 * 4, "l_0");
+static_assert(offsetof(mppib_racer_rigid_suspension_dyn_params, Jxx) == 64 + 33 * 4, "Jxx");
+static_assert(offsetof(mppib_racer_rigid_suspension_dyn_params, gear_sign) == 64 + 44 * 4, "gear_sign last");
+static_assert(sizeof(mppib_racer_rigid_suspension_dyn_params) == 244, "no padding");
 #endif
 
 /* Quadratic tracking cost on the RACER output vector (ours: the RACER cost classes are not in the reference tree,

@@ -114,6 +114,8 @@ static const PairEntry kPairs[] = {
                                                                                  MPPIB_COST_RACER_QUADRATIC),
   make_entry<plugins::RacerSuspensionLSTMDynamics, plugins::RacerQuadraticCost>(MPPIB_DYN_RACER_SUSPENSION_LSTM,
                                                                                 MPPIB_COST_RACER_QUADRATIC),
+  make_entry<plugins::RacerRigidSuspensionDynamics, plugins::RacerRigidQuadraticCost>(MPPIB_DYN_RACER_SUSPENSION,
+                                                                                      MPPIB_COST_RACER_QUADRATIC),
 };
 
 // RacerDubinsElevationLSTMSteering and RacerDubinsElevationSuspension with the steering LSTM on tensor cores (hidden_dim
@@ -1514,6 +1516,8 @@ int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, flo
         dyn_.data(), &net, is_set(MPPIB_BLOB_NORMALS_MAP) ? (const mppib_elevation_map_header*)normals_h_.data() : nullptr,
         x0, u, T, dt, states, outputs);
   }
+  if (dyn_id_ == MPPIB_DYN_RACER_SUSPENSION)
+    return mppib_host_output_trajectory_racer_rigid_suspension(dyn_.data(), x0, u, T, dt, states, outputs);
   if (dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION)
     return mppib_host_output_trajectory_racer_dubins_elevation(
         dyn_.data(), is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr, x0, u,

@@ -56,6 +56,8 @@ const mppib_control_limits* limits_of(int dyn_id, const void* p)
       return &((const mppib_racer_suspension_dyn_params*)p)->base.lim;
     case MPPIB_DYN_QUADROTOR:
       return &((const mppib_quadrotor_dyn_params*)p)->lim;
+    case MPPIB_DYN_RACER_SUSPENSION:
+      return &((const mppib_racer_rigid_suspension_dyn_params*)p)->lim;
   }
   return nullptr;
 }
@@ -1073,6 +1075,9 @@ int mppib_host_dims(int dyn_id, int* S, int* C, int* O)
     case MPPIB_DYN_QUADROTOR:
       s = 13, c = 4, o = 13;
       break;
+    case MPPIB_DYN_RACER_SUSPENSION:
+      s = 14, c = 2, o = 26;
+      break;
     default:
       return MPPIB_ERR_UNSUPPORTED;
   }
@@ -1114,6 +1119,8 @@ static int host_step_impl(int dyn_id, const void* dyn_params, const FnnT* nn, co
 int mppib_host_step(int dyn_id, const void* dyn_params, const float* nn_theta, const float* x, const float* u,
                     float dt, float* x_next, float* xdot, float* y)
 {
+  if (dyn_id == MPPIB_DYN_RACER_SUSPENSION)
+    return mppib_host_step_racer_rigid_suspension(dyn_params, x, u, dt, x_next, xdot, y);
   FnnT nn;
   if (dyn_id == MPPIB_DYN_AUTORALLY_NN && nn_theta)
     fnn_transpose(nn_theta, nn);
@@ -1187,6 +1194,8 @@ int mppib_host_output_trajectory(int dyn_id, const void* dyn_params, const float
     case MPPIB_DYN_QUADROTOR:
       return output_trajectory_impl<MPPIB_DYN_QUADROTOR, 13, 4, 13>(dyn_params, nullptr, *limits_of(dyn_id, dyn_params), x0,
                                                                    u, T, dt, states, outputs);
+    case MPPIB_DYN_RACER_SUSPENSION:
+      return mppib_host_output_trajectory_racer_rigid_suspension(dyn_params, x0, u, T, dt, states, outputs);
   }
   return MPPIB_ERR_UNSUPPORTED;
 }
@@ -1451,6 +1460,267 @@ int mppib_host_output_trajectory_lstm(const void* dyn_params, const mppib_host_l
     racer_step(p, &local, states + (size_t)t * S, ui, dt, xn.data(), xd.data(), y.data());
     memcpy(states + (size_t)(t + 1) * S, xn.data(), sizeof(float) * S);
     memcpy(outputs + (size_t)(t + 1) * O, y.data(), sizeof(float) * O);
+  }
+  return MPPIB_OK;
+}
+
+// ---- RacerSuspension host twin (dynamics/racer_suspension/racer_suspension.cu) ---------------------------------------
+// computeStateDeriv (:93-298) on the plane z = 0 with normal (0, 0, 1) (the map query is commented out, :128-135), in
+// float as the host body evaluates it, with the 3x3 omegaJacobian when jac != NULL (row-major [3][3]). Kept as written:
+// `f_r_B_i_Jac = R_C_i_to_B = f_r_C_i_Jac` (:215) is an assignment, so tau_jac takes the contact-frame Jacobian as if it
+// were the body-frame one; 1.0 / J is a double quotient rounded to float. The body-z velocity goes to BASELINK_VEL_B_Z,
+// not into BASELINK_VEL_B_X (DESIGN §8); ACCEL_X / ACCEL_Y / OMEGA_Z are 0.
+static void rigid_suspension_deriv(const mppib_racer_rigid_suspension_dyn_params& p, const float* x, const float* u,
+                                   float* xd, float* y, float* jac)
+{
+  typedef float M3[3][3];
+  const float qw = x[3], qx = x[4], qy = x[5], qz = x[6];
+  const float tx = 2.0f * qx, ty = 2.0f * qy, tz = 2.0f * qz;  // Eigen's Quaternion::toRotationMatrix
+  const float twx = tx * qw, twy = ty * qw, twz = tz * qw, txx = tx * qx, txy = ty * qx, txz = tz * qx;
+  const float tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+  const M3 R = { { 1.0f - (tyy + tzz), txy - twz, txz + twy },
+                 { txy + twz, 1.0f - (txx + tzz), tyz - twx },
+                 { txz - twy, tyz + twx, 1.0f - (txx + tyy) } };
+  const float* pI = x;
+  const float* v = x + 7;
+  const float* w = x + 10;
+  auto mul = [&](const float* a, float* out) {  // R a
+    for (int r = 0; r < 3; r++)
+      out[r] = R[r][0] * a[0] + R[r][1] * a[1] + R[r][2] * a[2];
+  };
+  auto mulT = [&](const float* a, float* out) {  // R^T a
+    for (int r = 0; r < 3; r++)
+      out[r] = R[0][r] * a[0] + R[1][r] * a[1] + R[2][r] * a[2];
+  };
+  auto cross = [](const float* a, const float* b, float* out) {
+    out[0] = a[1] * b[2] - a[2] * b[1];
+    out[1] = a[2] * b[0] - a[0] * b[2];
+    out[2] = a[0] * b[1] - a[1] * b[0];
+  };
+  const float tan_delta = tanf(x[13]);
+  float vb[3];
+  mulT(v, vb);
+  const float throttle = std::max(0.0f, u[0]), brake = std::max(0.0f, -u[0]);
+  const float acc = p.c_t * throttle - copysignf(p.c_b * brake, vb[0]) - p.c_v * vb[0] + p.c_0;
+  const float propulsion_force = p.mass * acc;
+
+  float f_B[3] = { 0, 0, 0 }, tau_B[3] = { 0, 0, 0 };
+  M3 tau_jac = {};
+  for (int i = 0; i < 4; i++)
+  {
+    float pb[3], Rpb[3], pw[3], wxp[3], Rwxp[3], pdot[3];
+    for (int r = 0; r < 3; r++)
+      pb[r] = p.wheel_pos_wrt_base_link[i][r] - p.cg_pos_wrt_base_link[r];
+    mul(pb, Rpb);
+    cross(w, pb, wxp);
+    mul(wxp, Rwxp);
+    for (int r = 0; r < 3; r++)
+    {
+      pw[r] = pI[r] + Rpb[r];
+      pdot[r] = v[r] + Rwxp[r];
+    }
+    // d pdot / d omega = R [e_k x pb]: column k
+    M3 pdot_jac;
+    for (int k = 0; k < 3; k++)
+    {
+      float e[3] = { 0, 0, 0 }, c[3], Rc[3];
+      e[k] = 1.0f;
+      cross(e, pb, c);
+      mul(c, Rc);
+      for (int r = 0; r < 3; r++)
+        pdot_jac[r][k] = Rc[r];
+    }
+    float f_k = -p.k_s[i] * (pw[2] - p.l_0[i]) - p.c_s[i] * pdot[2];
+    float f_k_jac[3] = { -p.c_s[i] * pdot_jac[2][0], -p.c_s[i] * pdot_jac[2][1], -p.c_s[i] * pdot_jac[2][2] };
+    if (f_k < 0)
+    {
+      f_k = 0;
+      f_k_jac[0] = f_k_jac[1] = f_k_jac[2] = 0;
+    }
+    float delta = 0.0f;
+    if (i == 0)
+      delta = atanf(p.wheel_base * tan_delta / (p.wheel_base - tan_delta * p.width / 2));
+    else if (i == 1)
+      delta = atanf(p.wheel_base * tan_delta / (p.wheel_base + tan_delta * p.width / 2));
+    const float n[3] = { R[2][0], R[2][1], R[2][2] };  // R^T (0, 0, 1)
+    const float wd[3] = { cosf(delta), sinf(delta), 0.0f };
+    float s[3], t[3];
+    cross(n, wd, s);
+    const float sn = sqrtf(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
+    for (int r = 0; r < 3; r++)
+      s[r] /= sn;
+    cross(s, n, t);
+    // contact velocity (pdot_x, pdot_y, 0) and its Jacobian (rows 0 and 1 of pdot_jac, row 2 zero) in the body frame
+    const float pdc[3] = { pdot[0], pdot[1], 0.0f };
+    float pdc_B[3];
+    mulT(pdc, pdc_B);
+    const float v_s = s[0] * pdc_B[0] + s[1] * pdc_B[1] + s[2] * pdc_B[2];
+    float v_s_jac[3];
+    for (int k = 0; k < 3; k++)
+    {
+      const float col[3] = { pdot_jac[0][k], pdot_jac[1][k], 0.0f };
+      float colB[3];
+      mulT(col, colB);
+      v_s_jac[k] = s[0] * colB[0] + s[1] * colB[1] + s[2] * colB[2];
+    }
+    const float f_n = f_k;
+    float mu_s = v_s / p.v_slip * p.mu, dmu = 0.0f;  // stribeck_friction (:77-91)
+    if (mu_s > p.mu)
+      mu_s = p.mu;
+    else if (mu_s < -p.mu)
+      mu_s = -p.mu;
+    else
+      dmu = p.mu / p.v_slip;
+    const float f_s = -mu_s * f_n;
+    const float f_t = std::max(-p.mu * f_n, std::min(propulsion_force / 4, p.mu * f_n));
+    float fc_jac[3][3];  // rows t, s, n of f_r_C_i_Jac
+    for (int k = 0; k < 3; k++)
+    {
+      fc_jac[0][k] = propulsion_force / 4 > p.mu * f_n ? p.mu * f_k_jac[k] :
+                     (propulsion_force / 4 < -p.mu * f_n ? -p.mu * f_k_jac[k] : 0.0f);
+      fc_jac[1][k] = -f_n * dmu * v_s_jac[k] - mu_s * f_k_jac[k];
+      fc_jac[2][k] = f_k_jac[k];
+    }
+    float f[3], pc[3];
+    for (int r = 0; r < 3; r++)
+      f[r] = t[r] * f_t + s[r] * f_s + n[r] * f_n;
+    const float dc[3] = { pw[0] - pI[0], pw[1] - pI[1], 0.0f - pI[2] };
+    mulT(dc, pc);
+    float tq[3];
+    cross(pc, f, tq);
+    for (int r = 0; r < 3; r++)
+    {
+      f_B[r] += f[r];
+      tau_B[r] += tq[r];
+    }
+    // tau_B_jac += -(f_r_B_i_Jac.colwise().cross(p_c_B_i)) with f_r_B_i_Jac = f_r_C_i_Jac (:215, as written)
+    for (int k = 0; k < 3; k++)
+    {
+      const float col[3] = { fc_jac[0][k], fc_jac[1][k], fc_jac[2][k] };
+      float c[3];
+      cross(col, pc, c);
+      for (int r = 0; r < 3; r++)
+        tau_jac[r][k] += -c[r];
+    }
+    y[11 + 2 * i] = pw[0];
+    y[12 + 2 * i] = pw[1];
+    y[19 + i] = sqrtf(f[0] * f[0] + f[1] * f[1] + f[2] * f[2]);
+  }
+
+  const float inv_mass = 1 / p.mass;
+  float Rf[3];
+  mul(f_B, Rf);
+  for (int r = 0; r < 3; r++)
+  {
+    xd[r] = v[r];
+    xd[7 + r] = inv_mass * Rf[r];
+  }
+  xd[9] += p.gravity;
+  xd[3] = 0.5f * (-qx * w[0] - qy * w[1] - qz * w[2]);
+  xd[4] = 0.5f * (qw * w[0] + qy * w[2] - qz * w[1]);
+  xd[5] = 0.5f * (qw * w[1] + qz * w[0] - qx * w[2]);
+  xd[6] = 0.5f * (qw * w[2] + qx * w[1] - qy * w[0]);
+  const float J[3] = { p.Jxx, p.Jyy, p.Jzz };
+  const float Jinv[3] = { (float)(1.0 / p.Jxx), (float)(1.0 / p.Jyy), (float)(1.0 / p.Jzz) };
+  const float Jw[3] = { J[0] * w[0], J[1] * w[1], J[2] * w[2] };
+  float Jwxw[3];
+  cross(Jw, w, Jwxw);
+  for (int r = 0; r < 3; r++)
+    xd[10 + r] = Jinv[r] * (Jwxw[r] + tau_B[r]);
+  if (jac)
+  {
+    // d(Jw x w)/dw, column k: (J e_k) x w - e_k x (J w)
+    for (int k = 0; k < 3; k++)
+    {
+      float e[3] = { 0, 0, 0 }, a[3], b[3];
+      e[k] = J[k];
+      cross(e, w, a);
+      e[k] = 1.0f;
+      cross(e, Jw, b);
+      for (int r = 0; r < 3; r++)
+        jac[r * 3 + k] = Jinv[r] * ((a[r] - b[r]) + tau_jac[r][k]);
+    }
+  }
+  xd[13] = p.steering_constant * (u[1] / p.steer_command_angle_scale - x[13]);
+
+  const float pbl[3] = { -p.cg_pos_wrt_base_link[0], -p.cg_pos_wrt_base_link[1], -p.cg_pos_wrt_base_link[2] };
+  float wxb[3], Rpbl[3];
+  cross(w, pbl, wxb);
+  mul(pbl, Rpbl);
+  for (int r = 0; r < 3; r++)
+  {
+    y[r] = vb[r] + wxb[r];
+    y[3 + r] = pI[r] + Rpbl[r];
+  }
+  // Quat2EulerNWU (math_utils.h:519-527)
+  y[7] = atan2f(2.0f * qz * qy + 2.0f * qw * qx, qw * qw + qz * qz - qy * qy - qx * qx);
+  y[8] = -asinf(fmaxf(-1.0f, fminf(-2.0f * qw * qy + 2.0f * qx * qz, 1.0f)));
+  y[6] = atan2f(2.0f * qy * qx + 2.0f * qz * qw, qw * qw + qx * qx - qy * qy - qz * qz);
+  y[9] = x[13];
+  y[10] = xd[13];
+  y[23] = y[24] = y[25] = 0.0f;
+}
+
+// step (host, :31-45): omega by approximate implicit Euler, (I - dt J_w)^-1 dt w_dot; the rest explicit; then q / |q|
+static void rigid_suspension_step(const mppib_racer_rigid_suspension_dyn_params& p, const float* x, const float* u, float dt,
+                                  float* xn, float* xd, float* y)
+{
+  float J[9];
+  rigid_suspension_deriv(p, x, u, xd, y, J);
+  float M[9];
+  for (int i = 0; i < 9; i++)
+    M[i] = (i % 4 == 0 ? 1.0f : 0.0f) - dt * J[i];
+  // the 3x3 inverse by cofactors, as Eigen computes it
+  const float c00 = M[4] * M[8] - M[5] * M[7], c01 = M[5] * M[6] - M[3] * M[8], c02 = M[3] * M[7] - M[4] * M[6];
+  const float det = M[0] * c00 + M[1] * c01 + M[2] * c02;
+  const float inv[9] = { c00 / det, (M[2] * M[7] - M[1] * M[8]) / det, (M[1] * M[5] - M[2] * M[4]) / det,
+                         c01 / det, (M[0] * M[8] - M[2] * M[6]) / det, (M[2] * M[3] - M[0] * M[5]) / det,
+                         c02 / det, (M[1] * M[6] - M[0] * M[7]) / det, (M[0] * M[4] - M[1] * M[3]) / det };
+  for (int i = 0; i < 14; i++)
+    xn[i] = x[i] + xd[i] * dt;
+  for (int r = 0; r < 3; r++)
+    xn[10 + r] = x[10 + r] + ((inv[r * 3] * dt) * xd[10] + (inv[r * 3 + 1] * dt) * xd[11] + (inv[r * 3 + 2] * dt) * xd[12]);
+  const float norm = sqrtf(xn[3] * xn[3] + xn[4] * xn[4] + xn[5] * xn[5] + xn[6] * xn[6]);
+  for (int i = 3; i < 7; i++)
+    xn[i] /= norm;
+}
+
+int mppib_host_state_deriv_racer_rigid_suspension(const void* dyn_params, const float* x, const float* u, float* xdot,
+                                                  float* y, float* omega_jacobian)
+{
+  if (!dyn_params || !x || !u || !xdot || !y)
+    return MPPIB_ERR_INVALID_ARG;
+  rigid_suspension_deriv(*(const mppib_racer_rigid_suspension_dyn_params*)dyn_params, x, u, xdot, y, omega_jacobian);
+  return MPPIB_OK;
+}
+
+int mppib_host_step_racer_rigid_suspension(const void* dyn_params, const float* x, const float* u, float dt, float* x_next,
+                                           float* xdot, float* y)
+{
+  if (!dyn_params || !x || !u || !x_next || !xdot || !y)
+    return MPPIB_ERR_INVALID_ARG;
+  rigid_suspension_step(*(const mppib_racer_rigid_suspension_dyn_params*)dyn_params, x, u, dt, x_next, xdot, y);
+  return MPPIB_OK;
+}
+
+int mppib_host_output_trajectory_racer_rigid_suspension(const void* dyn_params, const float* x0, const float* u, int T,
+                                                        float dt, float* states, float* outputs)
+{
+  // controller.cuh:643-663: outputs[0] from initializeDynamics (y <- x on the first 14 entries, the rest 0), then
+  // outputs[t + 1] = the outputs step t computes, which for this model are those of states[t]
+  if (!dyn_params || !x0 || !u || !states || !outputs || T <= 0)
+    return MPPIB_ERR_INVALID_ARG;
+  const int S = 14, C = 2, O = 26;
+  float xd[S], y[O] = {};
+  memcpy(states, x0, sizeof(float) * S);
+  memcpy(y, x0, sizeof(float) * S);
+  memcpy(outputs, y, sizeof(float) * O);
+  const auto& p = *(const mppib_racer_rigid_suspension_dyn_params*)dyn_params;
+  for (int t = 0; t < T - 1; t++)
+  {
+    float ui[2] = { u[(size_t)t * C], u[(size_t)t * C + 1] };
+    enforce(p.lim, ui, C);
+    rigid_suspension_step(p, states + (size_t)t * S, ui, dt, states + (size_t)(t + 1) * S, xd, outputs + (size_t)(t + 1) * O);
   }
   return MPPIB_OK;
 }

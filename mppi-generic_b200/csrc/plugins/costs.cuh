@@ -342,9 +342,13 @@ struct ARRobustCost : public Cost<ARRobustCost, mppib_ar_robust_cost_params>
 };
 
 // Quadratic tracking cost on the RACER output vector (ours, params.h: mppib_racer_quadratic_cost_params; the RACER cost
-// classes are not in the reference tree). Output indices: racer_dubins.cuh:35-76.
-struct RacerQuadraticCost : public Cost<RacerQuadraticCost, mppib_racer_quadratic_cost_params>
+// classes are not in the reference tree), at the output indices of BASELINK_VEL_B_X, BASELINK_POS_I_Y, YAW and
+// STEER_ANGLE of the model it is paired with. One cost id: the pair table picks the layout through the class.
+template <int VEL_X, int POS_Y, int YAW, int STEER>
+struct RacerQuadraticCostAt : public Cost<RacerQuadraticCostAt<VEL_X, POS_Y, YAW, STEER>, mppib_racer_quadratic_cost_params>
 {
+  using Params = mppib_racer_quadratic_cost_params;
+  using Aux = typename Cost<RacerQuadraticCostAt, Params>::Aux;
   __host__ __device__ static constexpr int sharedFloats(int T)
   {
     return T;
@@ -356,10 +360,10 @@ struct RacerQuadraticCost : public Cost<RacerQuadraticCost, mppib_racer_quadrati
   __device__ static __forceinline__ float computeStateCost(const Params& p, const Aux&, const float* theta_c,
                                                            const float* y, int t, int*)
   {
-    const float dv = y[0] - p.desired_speed;                   // BASELINK_VEL_B_X
-    const float dyaw = normalizeAngle(y[5] - p.desired_yaw);   // YAW
-    const float dy = y[3] - p.desired_y;                       // BASELINK_POS_I_Y
-    const float st = y[8];                                     // STEER_ANGLE
+    const float dv = y[VEL_X] - p.desired_speed;
+    const float dyaw = normalizeAngle(y[YAW] - p.desired_yaw);
+    const float dy = y[POS_Y] - p.desired_y;
+    const float st = y[STEER];
     const float cost =
         p.speed_coeff * dv * dv + p.yaw_coeff * dyaw * dyaw + p.lateral_coeff * dy * dy + p.steer_coeff * st * st;
     return cost * theta_c[t];
@@ -368,6 +372,14 @@ struct RacerQuadraticCost : public Cost<RacerQuadraticCost, mppib_racer_quadrati
   {
     return 0.0f;
   }
+};
+// the RACER-Dubins output layout, racer_dubins.cuh:35-76 (every RACER model but the rigid body)
+struct RacerQuadraticCost : RacerQuadraticCostAt<0, 3, 5, 8>
+{
+};
+// RacerSuspension's output layout, racer_suspension.cuh:36-65
+struct RacerRigidQuadraticCost : RacerQuadraticCostAt<0, 4, 6, 9>
+{
 };
 
 // cost_functions/quadrotor/quadrotor_quadratic_cost.cu:70-132 (device body) with the float-array quaternion helpers of
@@ -538,10 +550,8 @@ struct QuadrotorMapCost : public Cost<QuadrotorMapCost, mppib_quadrotor_map_cost
   // :199-208: roll and pitch of Quat2EulerNWU
   __device__ static __forceinline__ float computeStabilizingCost(const Params& p, const float* s)
   {
-    const float* q = s + 6;
-    const float roll = atan2f(2.0f * q[3] * q[2] + 2.0f * q[0] * q[1], q[0] * q[0] + q[3] * q[3] - q[2] * q[2] - q[1] * q[1]);
-    const float temp = -2.0f * q[0] * q[2] + 2.0f * q[1] * q[3];
-    const float pitch = -asinf(fmaxf(fminf(1.0f, temp), -1.0f));
+    float roll, pitch, yaw;
+    quat2EulerNWU(s + 6, roll, pitch, yaw);
     return p.attitude_coeff * (MPPIB_SQ(roll) + MPPIB_SQ(pitch));
   }
   // :92-144. computeWaypointCost is evaluated but not added on the device, so it is not computed here. A non-zero gate

@@ -1565,6 +1565,181 @@ struct RacerDubinsElevationDynamics
   }
 };
 
+// ---- RacerSuspension: dynamics/racer_suspension/racer_suspension.cu:55-75 (device updateState), :93-298 (computeStateDeriv),
+//      :300-306 (device step) --------------------------------------------------------------------------------------------
+// The 6-DoF rigid-body RACER vehicle: quaternion attitude, body rates through Euler's equations, four spring-damper
+// wheels with Stribeck side friction and a traction force limited by friction. The reference's elevation query is
+// commented out (:128-135), so every wheel stands on the plane z = 0 with normal (0, 0, 1), and the terms of the body that
+// only a tilted normal makes non-zero (h_dot, the normal's x / y) are left out. The host twin (host_twins.cpp) keeps the
+// reference's host step: ω by approximate implicit Euler through the as-written Jacobian. This is the device one: explicit
+// Euler on all 14 states. Divisions use rcp_nr (within 1 ulp of the quotient): 1 / mass, 1 / J (the reference's
+// 1.0 / Jxx in double, rounded to float), the contact frame's 1 / |n x w| and the quaternion's 1 / |q|.
+struct RacerRigidSuspensionDynamics
+    : public Dynamics<RacerRigidSuspensionDynamics, mppib_racer_rigid_suspension_dyn_params, 14, 2, 26>
+{
+  enum
+  {
+    P_I_X = 0, P_I_Y, P_I_Z, Q_W, Q_X, Q_Y, Q_Z, V_I_X, V_I_Y, V_I_Z, OMEGA_B_X, OMEGA_B_Y, OMEGA_B_Z, STEER_ANGLE
+  };
+  enum
+  {
+    O_VEL_B_X = 0, O_POS_I_X = 3, O_YAW = 6, O_ROLL, O_PITCH, O_STEER_ANGLE, O_STEER_ANGLE_RATE, O_WHEEL_POS = 11,
+    O_WHEEL_FORCE = 19, O_ACCEL_X = 23, O_ACCEL_Y, O_OMEGA_Z
+  };
+  static constexpr bool UNROLL_STEPS = false;
+  // dynamics.cuh:429-435; the outputs past the state, which the reference leaves as it finds them, start at 0
+  __device__ static __forceinline__ void initializeDynamics(const Params&, const Aux&, float*, Carry&, const float* x,
+                                                            float* y)
+  {
+#pragma unroll
+    for (int i = 0; i < 26; i++)
+      y[i] = i < 14 ? x[i] : 0.0f;
+  }
+
+  // computeStateDeriv on flat ground: xdot of all 14 states, and the outputs of x (not of the next state)
+  __device__ static __forceinline__ void stateDerivAndOutput(const Params& p, const float* x, const float* u, float* xd,
+                                                             float* y)
+  {
+    const float qw = x[Q_W], qx = x[Q_X], qy = x[Q_Y], qz = x[Q_Z];
+    // Eigen's Quaternion::toRotationMatrix
+    const float tx = 2.0f * qx, ty = 2.0f * qy, tz = 2.0f * qz;
+    const float twx = tx * qw, twy = ty * qw, twz = tz * qw, txx = tx * qx, txy = ty * qx, txz = tz * qx;
+    const float tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+    const float R[3][3] = { { 1.0f - (tyy + tzz), txy - twz, txz + twy },
+                            { txy + twz, 1.0f - (txx + tzz), tyz - twx },
+                            { txz - twy, tyz + twx, 1.0f - (txx + tyy) } };
+    const float* v = x + V_I_X;
+    const float* w = x + OMEGA_B_X;
+    const float tan_delta = tanf(x[STEER_ANGLE]);
+    // the body-frame velocity of the CG, R^T v
+    float vb[3];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+      vb[i] = R[0][i] * v[0] + R[1][i] * v[1] + R[2][i] * v[2];
+
+    // linear engine model (:108-113); copysign keeps the sign of a zero vel_x
+    const float throttle = fmaxf(0.0f, u[0]), brake = fmaxf(0.0f, -u[0]);
+    const float acc = p.c_t * throttle - copysignf(p.c_b * brake, vb[0]) - p.c_v * vb[0] + p.c_0;
+    const float propulsion_force = p.mass * acc;
+
+    float f_B[3] = { 0.0f, 0.0f, 0.0f }, tau_B[3] = { 0.0f, 0.0f, 0.0f };
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+    {
+      // wheel position relative to the CG, in the body and the world frame; its world velocity v + R (w x p)
+      const float pb[3] = { p.wheel_pos_wrt_base_link[i][0] - p.cg_pos_wrt_base_link[0],
+                            p.wheel_pos_wrt_base_link[i][1] - p.cg_pos_wrt_base_link[1],
+                            p.wheel_pos_wrt_base_link[i][2] - p.cg_pos_wrt_base_link[2] };
+      const float wxp[3] = { w[1] * pb[2] - w[2] * pb[1], w[2] * pb[0] - w[0] * pb[2], w[0] * pb[1] - w[1] * pb[0] };
+      float pw[3], pdot[3];
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+      {
+        pw[r] = x[P_I_X + r] + (R[r][0] * pb[0] + R[r][1] * pb[1] + R[r][2] * pb[2]);
+        pdot[r] = v[r] + (R[r][0] * wxp[0] + R[r][1] * wxp[1] + R[r][2] * wxp[2]);
+      }
+      // spring-damper on the spring length above the ground z = 0, clamped at 0 (wheel lift)
+      float f_n = -p.k_s[i] * (pw[2] - p.l_0[i]) - p.c_s[i] * pdot[2];
+      if (f_n < 0.0f)
+        f_n = 0.0f;
+      // Ackermann angle of the front wheels
+      float delta = 0.0f;
+      if (i == 0)
+        delta = atanf(p.wheel_base * tan_delta / (p.wheel_base - tan_delta * p.width / 2));
+      else if (i == 1)
+        delta = atanf(p.wheel_base * tan_delta / (p.wheel_base + tan_delta * p.width / 2));
+      float sd, cd;
+      sincosf(delta, &sd, &cd);
+      // contact frame: n = R^T (0, 0, 1), s = normalised n x (cos d, sin d, 0), t = s x n
+      const float n[3] = { R[2][0], R[2][1], R[2][2] };
+      float s[3] = { -n[2] * sd, n[2] * cd, n[0] * sd - n[1] * cd };
+      const float inv_s = rcp_nr(sqrtf(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]));
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+        s[r] *= inv_s;
+      const float t[3] = { s[1] * n[2] - s[2] * n[1], s[2] * n[0] - s[0] * n[2], s[0] * n[1] - s[1] * n[0] };
+      // side slip velocity s . R^T (pdot_x, pdot_y, 0), Stribeck friction, traction clamped at +-mu f_n
+      float v_s = 0.0f;
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+        v_s += s[r] * (R[0][r] * pdot[0] + R[1][r] * pdot[1]);
+      float mu_s = v_s / p.v_slip * p.mu;
+      mu_s = mu_s > p.mu ? p.mu : (mu_s < -p.mu ? -p.mu : mu_s);
+      const float f_s = -mu_s * f_n;
+      const float f_t = fmaxf(-p.mu * f_n, fminf(propulsion_force / 4, p.mu * f_n));
+      const float f[3] = { t[0] * f_t + s[0] * f_s + n[0] * f_n, t[1] * f_t + s[1] * f_s + n[1] * f_n,
+                           t[2] * f_t + s[2] * f_s + n[2] * f_n };
+      // contact point in the body frame: R^T ((pw_x, pw_y, 0) - p_I)
+      const float dc[3] = { pw[0] - x[P_I_X], pw[1] - x[P_I_Y], -x[P_I_Z] };
+      float pc[3];
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+        pc[r] = R[0][r] * dc[0] + R[1][r] * dc[1] + R[2][r] * dc[2];
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+        f_B[r] += f[r];
+      tau_B[0] += pc[1] * f[2] - pc[2] * f[1];
+      tau_B[1] += pc[2] * f[0] - pc[0] * f[2];
+      tau_B[2] += pc[0] * f[1] - pc[1] * f[0];
+      y[O_WHEEL_POS + 2 * i] = pw[0];
+      y[O_WHEEL_POS + 2 * i + 1] = pw[1];
+      y[O_WHEEL_FORCE + i] = sqrtf(f[0] * f[0] + f[1] * f[1] + f[2] * f[2]);
+    }
+
+    // v_dot = R f / m + g, q_dot = q (x) (0, w) / 2, w_dot = J^-1 (J w x w + tau)
+    const float inv_mass = rcp_nr(p.mass);
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+    {
+      xd[P_I_X + r] = v[r];
+      xd[V_I_X + r] = inv_mass * (R[r][0] * f_B[0] + R[r][1] * f_B[1] + R[r][2] * f_B[2]);
+    }
+    xd[V_I_Z] += p.gravity;
+    xd[Q_W] = 0.5f * (-qx * w[0] - qy * w[1] - qz * w[2]);
+    xd[Q_X] = 0.5f * (qw * w[0] + qy * w[2] - qz * w[1]);
+    xd[Q_Y] = 0.5f * (qw * w[1] + qz * w[0] - qx * w[2]);
+    xd[Q_Z] = 0.5f * (qw * w[2] + qx * w[1] - qy * w[0]);
+    const float Jw[3] = { p.Jxx * w[0], p.Jyy * w[1], p.Jzz * w[2] };
+    xd[OMEGA_B_X] = rcp_nr(p.Jxx) * ((Jw[1] * w[2] - Jw[2] * w[1]) + tau_B[0]);
+    xd[OMEGA_B_Y] = rcp_nr(p.Jyy) * ((Jw[2] * w[0] - Jw[0] * w[2]) + tau_B[1]);
+    xd[OMEGA_B_Z] = rcp_nr(p.Jzz) * ((Jw[0] * w[1] - Jw[1] * w[0]) + tau_B[2]);
+    // first-order steering lag (:253-255)
+    xd[STEER_ANGLE] = p.steering_constant * (u[1] / p.steer_command_angle_scale - x[STEER_ANGLE]);
+
+    // outputs (:257-297). BASELINK_VEL_B_Y / _Z get their own components: the reference writes all three into
+    // BASELINK_VEL_B_X (DESIGN §8). ACCEL_X, ACCEL_Y and OMEGA_Z are 0.
+    const float cg[3] = { p.cg_pos_wrt_base_link[0], p.cg_pos_wrt_base_link[1], p.cg_pos_wrt_base_link[2] };
+    y[O_VEL_B_X + 0] = vb[0] + (w[1] * -cg[2] - w[2] * -cg[1]);
+    y[O_VEL_B_X + 1] = vb[1] + (w[2] * -cg[0] - w[0] * -cg[2]);
+    y[O_VEL_B_X + 2] = vb[2] + (w[0] * -cg[1] - w[1] * -cg[0]);
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+      y[O_POS_I_X + r] = x[P_I_X + r] + (R[r][0] * -cg[0] + R[r][1] * -cg[1] + R[r][2] * -cg[2]);
+    quat2EulerNWU(x + Q_W, y[O_ROLL], y[O_PITCH], y[O_YAW]);
+    y[O_STEER_ANGLE] = x[STEER_ANGLE];
+    y[O_STEER_ANGLE_RATE] = xd[STEER_ANGLE];
+    y[O_ACCEL_X] = 0.0f;
+    y[O_ACCEL_Y] = 0.0f;
+    y[O_OMEGA_Z] = 0.0f;
+  }
+
+  // :300-306 with :55-75: the outputs are those of the state passed in, so the cost of step t sees x_t
+  // (mppi_common.cu:118-127); then explicit Euler and q / |q|
+  __device__ static __forceinline__ void step(const Params& p, const Aux&, float*, Carry&, const float* x, float* x_next,
+                                              float* xd, const float* u, float* y, int /*t*/, float dt)
+  {
+    stateDerivAndOutput(p, x, u, xd, y);
+#pragma unroll
+    for (int i = 0; i < 14; i++)
+      x_next[i] = x[i] + xd[i] * dt;
+    float* q = x_next + Q_W;
+    const float inv = rcp_nr(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]));
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+      q[i] *= inv;
+  }
+};
+
 // ---- Quadrotor: dynamics/quadrotor/quadrotor_dynamics.cu:124-179 (device computeDynamics + updateState) with
 //      Quat2DCM / omega2edot of utils/math_utils.h:272-283,534-540 ------------------------------------------------------
 // The only in-tree model with CONTROL_DIM = 4: one 16-byte noise group is one time step (rollout_kernel.cuh).

@@ -30,6 +30,7 @@ FLT_MAX = 3.4028234663852886e38
 DYN_CARTPOLE, DYN_DOUBLE_INTEGRATOR, DYN_AUTORALLY_NN, DYN_RACER_LSTM, DYN_QUADROTOR = 0, 1, 2, 3, 4
 DYN_RACER_DUBINS_ELEVATION = 5
 DYN_RACER_SUSPENSION_LSTM = 6
+DYN_RACER_SUSPENSION = 7
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
 COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
 COST_QUADROTOR_MAP = 7
@@ -168,6 +169,31 @@ class RacerSuspensionDynParams(C.Structure):
     _fields_ = RacerLSTMDynParams._fields_ + [("spring_k", C.c_float), ("drag_c", C.c_float), ("mass", C.c_float),
                                               ("I_xx", C.c_float), ("I_yy", C.c_float), ("wheel_radius", C.c_float),
                                               ("c_g", C.c_float * 3)]
+
+
+class RacerRigidSuspensionDynParams(C.Structure):
+    """mppib_racer_rigid_suspension_dyn_params (params.h): RacerSuspensionParams (racer_suspension.cuh:8-128) field for
+    field, float3 as three floats, the derived fields included."""
+    _fields_ = [("lim", ControlLimits), ("wheel_radius", C.c_float), ("mass", C.c_float), ("wheel_base", C.c_float),
+                ("width", C.c_float), ("height", C.c_float), ("gravity", C.c_float), ("k_s", C.c_float * 4),
+                ("c_s", C.c_float * 4), ("l_0", C.c_float * 4), ("cg_pos_wrt_base_link", C.c_float * 3),
+                ("wheel_pos_wrt_base_link", (C.c_float * 3) * 4), ("Jxx", C.c_float), ("Jyy", C.c_float),
+                ("Jzz", C.c_float), ("mu", C.c_float), ("v_slip", C.c_float), ("c_t", C.c_float), ("c_b", C.c_float),
+                ("c_v", C.c_float), ("c_0", C.c_float), ("steering_constant", C.c_float),
+                ("steer_command_angle_scale", C.c_float), ("gear_sign", C.c_int)]
+
+    def recalcParams(self) -> None:
+        """RacerSuspensionParams::recalcParams (racer_suspension.cuh:113-127): the float expressions as the reference's
+        types evaluate them, the inertias in double."""
+        f32 = np.float32
+        wb, w, h, m, g = f32(self.wheel_base), f32(self.width), f32(self.height), f32(self.mass), f32(self.gravity)
+        self.cg_pos_wrt_base_link[:] = [wb / f32(2), 0.0, f32(0.2)]
+        for i in range(4):
+            self.l_0[i] = f32(self.wheel_radius) + m / f32(4) * -g / f32(self.k_s[i])
+        for i, (x, y) in enumerate(((wb, w / f32(2)), (wb, -w / f32(2)), (0.0, w / f32(2)), (0.0, -w / f32(2)))):
+            self.wheel_pos_wrt_base_link[i][:] = [x, y, 0.0]
+        d = lambda a, b: 1.0 / 12 * float(m) * float(f32(a * a + b * b))  # noqa: E731
+        self.Jxx, self.Jyy, self.Jzz = d(h, w), d(h, wb), d(wb, w)
 
 
 class RacerQuadraticCostParams(C.Structure):
@@ -353,6 +379,8 @@ ABI_SYMBOLS = [
     "mppib_host_step_racer_dubins_elevation", "mppib_host_output_trajectory_racer_dubins_elevation",
     "mppib_host_grad_racer_dubins_elevation", "mppib_host_step_racer_suspension",
     "mppib_host_output_trajectory_racer_suspension", "mppib_host_normals_at_world_pose",
+    "mppib_host_state_deriv_racer_rigid_suspension", "mppib_host_step_racer_rigid_suspension",
+    "mppib_host_output_trajectory_racer_rigid_suspension",
     "mppib_host_elevation_at_world_pose", "mppib_host_static_settling", "mppib_host_lstm_initialize",
     "mppib_set_rmppi", "mppib_init_eval", "mppib_set_tsallis", "mppib_sample_trajectories", "mppib_nominal_trajectory", "mppib_compute_control", "mppib_host_npz_read", "mppib_comm_p2p_handle", "mppib_comm_p2p_open", "mppib_host_rmppi_line_search_weights", "mppib_host_rmppi_candidates",
     "mppib_host_rmppi_best_index", "mppib_set_ddp", "mppib_ddp_feedback",
@@ -427,6 +455,9 @@ def lib() -> C.CDLL:
     L.mppib_host_step_racer_suspension.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, vp, C.c_float, vp, vp, vp]
     L.mppib_host_output_trajectory_racer_suspension.argtypes = [vp, C.POINTER(HostLSTM), vp, vp, vp, C.c_int, C.c_float,
                                                                  vp, vp]
+    L.mppib_host_state_deriv_racer_rigid_suspension.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.mppib_host_step_racer_rigid_suspension.argtypes = [vp, vp, vp, C.c_float, vp, vp, vp]
+    L.mppib_host_output_trajectory_racer_rigid_suspension.argtypes = [vp, vp, vp, C.c_int, C.c_float, vp, vp]
     L.mppib_set_rmppi.argtypes = [vp, C.c_float, vp]
     L.mppib_set_tsallis.argtypes = [vp, C.c_float, C.c_float]
     L.mppib_init_eval.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]
@@ -1078,6 +1109,136 @@ class RacerDubinsElevationSuspension(RacerDubinsElevationLSTMSteering):
         _check(lib().mppib_host_output_trajectory_racer_suspension(C.addressof(self.params), C.byref(net),
                                                                    self._normals_ptr(), _ptr(_f32(x0)), _ptr(_f32(u)), T,
                                                                    C.c_float(dt), _ptr(states), _ptr(outputs)))
+
+
+class RacerSuspension(_Dynamics):
+    """dynamics/racer_suspension/racer_suspension.cuh — RacerSuspension() / RacerSuspension(params): the 6-DoF rigid-body
+    RACER vehicle (S14 C2 O26) on four spring-damper wheels over the plane z = 0. Its blob is RacerSuspensionParams
+    (params.h: mppib_racer_rigid_suspension_dyn_params); call ``params.recalcParams()`` after changing a base field. The
+    texture helper exists for API compatibility: the model reads no map."""
+    DYN_ID, STATE_DIM, CONTROL_DIM, OUTPUT_DIM = DYN_RACER_SUSPENSION, 14, 2, 26
+    P_I_X, P_I_Y, P_I_Z, ATTITUDE_QW, V_I_X, OMEGA_B_X, STEER_ANGLE = 0, 1, 2, 3, 7, 10, 13
+    BASELINK_VEL_B_X, BASELINK_POS_I_Y, YAW, ROLL, PITCH, OUT_STEER_ANGLE = 0, 4, 6, 7, 8, 9
+
+    def __init__(self, params: Optional[RacerRigidSuspensionDynParams] = None):
+        super().__init__()
+        p = RacerRigidSuspensionDynParams()
+        p.lim.set_defaults()
+        # racer_suspension.cuh:70-111
+        p.wheel_radius, p.mass, p.wheel_base, p.width, p.height, p.gravity = 0.32, 1447.0, 2.981, 1.5, 1.5, -9.81
+        for i in range(4):
+            p.k_s[i], p.c_s[i] = 14000.0, 2000.0
+        p.mu, p.v_slip = 0.65, 0.1
+        p.c_t, p.c_b, p.c_v, p.c_0 = 3.0, 10.0, 0.2, 0.0
+        p.steering_constant, p.steer_command_angle_scale, p.gear_sign = 0.6, -2.45, 1
+        p.recalcParams()
+        self.params = p
+        if params is not None:
+            self.setParams(params)
+        self.tex_helper_ = TwoDTextureHelper()
+
+    def getParams(self) -> RacerRigidSuspensionDynParams:
+        out = RacerRigidSuspensionDynParams()
+        C.memmove(C.byref(out), C.byref(self.params), C.sizeof(RacerRigidSuspensionDynParams))
+        return out
+
+    def setParams(self, params: RacerRigidSuspensionDynParams) -> None:
+        C.memmove(C.byref(self.params), C.byref(params), C.sizeof(RacerRigidSuspensionDynParams))
+
+    def getTextureHelper(self) -> "TwoDTextureHelper":
+        return self.tex_helper_
+
+    def getZeroState(self) -> np.ndarray:
+        z = np.zeros(self.STATE_DIM, dtype=np.float32)
+        z[self.ATTITUDE_QW] = 1.0
+        return z
+
+    def restHeight(self) -> float:
+        """P_I_Z of the car upright at rest in equilibrium: each spring is wheel_radius long, compressed from its rest length
+        l_0 by mass / 4 * (-gravity) / k_s, so the four spring forces carry the weight."""
+        return float(np.float32(self.params.wheel_radius) + np.float32(self.params.cg_pos_wrt_base_link[2]))
+
+    def computeStateDeriv(self, state, control, omega_jacobian: bool = False):
+        """Host computeStateDeriv (racer_suspension.cu:93-298): returns (state_der, output[, omegaJacobian 3x3])."""
+        xd, y, J = np.zeros(14, np.float32), np.zeros(26, np.float32), np.zeros((3, 3), np.float32)
+        _check(lib().mppib_host_state_deriv_racer_rigid_suspension(C.addressof(self.params), _ptr(_f32(state)),
+                                                                    _ptr(_f32(control)), _ptr(xd), _ptr(y),
+                                                                    _ptr(J) if omega_jacobian else None))
+        return (xd, y, J) if omega_jacobian else (xd, y)
+
+    def step(self, state, control, dt: float):
+        """Host step (racer_suspension.cu:31-45): returns (next_state, state_der, output of `state`)."""
+        xn, xd, y = np.zeros(14, np.float32), np.zeros(14, np.float32), np.zeros(26, np.float32)
+        _check(lib().mppib_host_step_racer_rigid_suspension(C.addressof(self.params), _ptr(_f32(state)), _ptr(_f32(control)),
+                                                             dt, _ptr(xn), _ptr(xd), _ptr(y)))
+        return xn, xd, y
+
+    def updateState(self, state, state_der, dt: float) -> np.ndarray:
+        """racer_suspension.cu:47-53: explicit Euler, then q / |q|."""
+        xn = (_f32(state) + _f32(state_der) * np.float32(dt)).astype(np.float32)
+        q = xn[3:7]
+        xn[3:7] = q / np.float32(np.sqrt(np.float32(np.dot(q, q))))
+        return xn
+
+    def output_trajectory(self, x0, u, T: int, dt: float, states: np.ndarray, outputs: np.ndarray) -> None:
+        _check(lib().mppib_host_output_trajectory_racer_rigid_suspension(C.addressof(self.params), _ptr(_f32(x0)),
+                                                                          _ptr(_f32(u)), T, dt, _ptr(states),
+                                                                          _ptr(outputs)))
+
+    def enforceLeash(self, state_true, state_nominal, leash_values) -> np.ndarray:
+        """RacerSuspension::enforceLeash (racer_suspension.cu:389-447): x / y in the body frame of the true state's yaw, the
+        quaternion left as state_true has it, the other states component-wise."""
+        t, n, l = _f32(state_true), _f32(state_nominal), _f32(leash_values)
+        f32 = np.float32
+        qw, qx, qy, qz = (float(v) for v in t[3:7])
+        yaw = f32(math.atan2(2 * qy * qx + 2 * qz * qw, qw * qw + qx * qx - qy * qy - qz * qz))
+        cy, sy = f32(math.cos(yaw)), f32(math.sin(yaw))
+        out = t.copy()
+        dx, dy = n[0] - t[0], n[1] - t[1]
+        dxb = np.clip(dx * cy + dy * sy, -l[0], l[0])
+        dyb = np.clip(-dx * sy + dy * cy, -l[1], l[1])
+        out[0] += dxb * cy + -dyb * sy
+        out[1] += dxb * sy + dyb * cy
+        for i in range(2, 14):
+            if 3 <= i < 7:
+                continue
+            d = n[i] - t[i]
+            out[i] = t[i] + np.clip(d, -l[i], l[i]) if l[i] < abs(d) else n[i]
+        return out.astype(np.float32)
+
+    @staticmethod
+    def _rotate(q, v):
+        w, x, y, z = (float(c) for c in q)
+        R = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                      [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                      [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+        return R @ np.asarray(v, np.float64)
+
+    def attitudeFromState(self, state) -> np.ndarray:
+        """(w, x, y, z)"""
+        return _f32(state)[3:7].copy()
+
+    def positionFromState(self, state) -> np.ndarray:
+        s = _f32(state)
+        return (s[0:3] - self._rotate(s[3:7], list(self.params.cg_pos_wrt_base_link))).astype(np.float32)
+
+    def velocityFromState(self, state) -> np.ndarray:
+        s = _f32(state)
+        q = s[3:7] * np.array([1, -1, -1, -1], np.float32)
+        v_B = self._rotate(q, s[7:10])
+        return (v_B + np.cross(s[10:13], -np.array(list(self.params.cg_pos_wrt_base_link)))).astype(np.float32)
+
+    def angularRateFromState(self, state) -> np.ndarray:
+        return _f32(state)[10:13].copy()
+
+    def stateFromOdometry(self, q_B_to_I, pos_base_link_I, vel_base_link_B, omega_B) -> np.ndarray:
+        s = np.zeros(14, np.float32)
+        s[3:7] = q_B_to_I
+        s[10:13] = omega_B
+        cg = np.array(list(self.params.cg_pos_wrt_base_link), np.float64)
+        s[0:3] = np.asarray(pos_base_link_I) + self._rotate(q_B_to_I, cg)
+        s[7:10] = self._rotate(q_B_to_I, np.asarray(vel_base_link_B) + np.cross(omega_B, cg))
+        return s
 
 
 class _Cost:

@@ -431,3 +431,24 @@ def by_name(name: str, N: Optional[int] = None, T: Optional[int] = None) -> Work
     if T is not None:
         kw["T"] = T
     return BUILDERS[name](**kw)
+
+
+def racer_rigid_suspension(N: int = 32768, T: int = 100, D: int = 1, colored: bool = False) -> Workload:
+    """RacerSuspension (the rigid-body RACER vehicle, reference default parameters) + our quadratic tracking cost: from rest,
+    upright at its equilibrium height (every spring at its rest length), drive at 5 m/s along +x. dt = 0.01: in the slip band
+    the side friction's yaw eigenvalue is near -150 1/s, so the device's explicit step is stable only below about 0.013 s
+    (DESIGN §8). D = 2: Tube-MPPI / RMPPI (nominal and real system). N and T as tools/racer_elevation_timing.py."""
+    dyn = H.RacerSuspension()
+    dyn.setControlRanges([(-1.0, 1.0), (-1.0, 1.0)])  # throttle/brake, steering command
+    cost = H.RacerQuadraticCost()
+    cost.params.desired_speed = 5.0
+    if colored:
+        sampler = H.ColoredNoiseDistribution(2, [0.3, 0.3], [1.0, 1.0])
+    else:
+        sampler = H.GaussianDistribution(2, [0.3, 0.3])
+    x0 = np.tile(dyn.getZeroState(), (D, 1))
+    x0[:, dyn.P_I_Z] = dyn.restHeight()
+    U0 = np.zeros((D, T, 2), np.float32)
+    name = f"racer_rigid_suspension{'_tube' if D == 2 else ''}{'_colored' if colored else ''}_N{N}_T{T}"
+    return Workload(name, "tube" if D == 2 else "vanilla", dyn, cost, sampler, N, T, D, 0.01, 1.0, 0.0, x0, U0,
+                    extra={"nominal_threshold": 20.0} if D == 2 else {})
