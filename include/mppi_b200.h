@@ -130,6 +130,12 @@ int mppib_seed(mppib_engine* e, unsigned long long seed, unsigned long long offs
 int mppib_burn_draws(mppib_engine* e, int n_generate_calls);
 /* Current absolute RNG offset in normals (checkpoint/resume: SURVEY §5). */
 int mppib_get_rng_offset(mppib_engine* e, unsigned long long* offset);
+/* MPPIB_SAMPLER_SMOOTH_MPPI: the rate mean [T][C] the sampler carries from solve to solve (deriv_action_mean_d_,
+ * smooth-MPPI.cuh), zero at mppib_create. Each solve samples its rates around row min(optimization_stride, T - 1) and its
+ * merge replaces the whole array; mppib_burn_draws broadcasts row min(1, T - 1). get returns it once the solves enqueued
+ * so far are done; set while a solve is pending returns MPPIB_ERR_STATE. Other samplers: MPPIB_ERR_INVALID_ARG. */
+int mppib_get_derivative_mean(mppib_engine* e, float* host);
+int mppib_set_derivative_mean(mppib_engine* e, const float* host);
 /* Join an NCCL communicator for world_size > 1. unique_id = the 128-byte ncclUniqueId created on rank 0 and
  * distributed by the caller (torch.distributed / MPI / a file). No reference counterpart (single GPU only). */
 int mppib_comm_unique_id(void* unique_id_128);

@@ -48,7 +48,9 @@ enum mppib_sampler_id
 {
   MPPIB_SAMPLER_GAUSSIAN = 0,     /* sampling_distributions/gaussian/gaussian.cuh */
   MPPIB_SAMPLER_COLORED_NOISE = 1, /* sampling_distributions/colored_noise/colored_noise.cuh */
-  MPPIB_SAMPLER_NLN = 2            /* sampling_distributions/nln/nln.cuh: normal x log-normal noise, GaussianParams */
+  MPPIB_SAMPLER_NLN = 2,           /* sampling_distributions/nln/nln.cuh: normal x log-normal noise, GaussianParams */
+  MPPIB_SAMPLER_SMOOTH_MPPI = 3    /* sampling_distributions/smooth-MPPI/smooth-MPPI.cuh: sampled control rates,
+                                      mppib_smooth_mppi_params */
 };
 
 /* ---- Dynamics base: control limits (dynamics/dynamics.cuh:133,511-512) ------------------------- */
@@ -397,6 +399,15 @@ typedef struct mppib_gaussian_params
   float offset_decay_rate;                                          /* 0.97 */
   float fmin;                                                       /* 0.0 */
 } mppib_gaussian_params;
+
+/* SmoothMPPIParams (smooth-MPPI.cuh:15-24): the Gaussian blob, then the sampler's own integration step. The rates are
+ * sampled with the Gaussian fields; a control is mu + rate * dt. The blob of MPPIB_BLOB_SAMPLER_PARAMS on a
+ * MPPIB_SAMPLER_SMOOTH_MPPI engine. */
+typedef struct mppib_smooth_mppi_params
+{
+  mppib_gaussian_params gaussian;
+  float dt; /* 0.015 (smooth-MPPI.cuh:21); not the controller's dt */
+} mppib_smooth_mppi_params;
 
 #ifdef __cplusplus
 }

@@ -26,12 +26,22 @@ constexpr int kCombineCols = 32;     // one warp-width of columns per block: 128
 constexpr int kCombineGroups = 16;   // 16 warps split the records
 constexpr int kCombineMaxRecords = 4096;
 
-__global__ void __launch_bounds__(kCombineCols* kCombineGroups)
-    combine_kernel(const float* __restrict__ records,   // [nrec][D][pstride]  (V at [kPartialHeader..))
-                   const float4* __restrict__ headers,  // [nrec][D] (beta_b, eta_b, sum w^2_b, -)
-                   int nrec, int D, int TC, int pstride, float lambda_inv, int normalize,
-                   float* __restrict__ out,    // [D][pstride] (device)
-                   float* __restrict__ out2)   // optional second copy (mapped host result), may be nullptr
+constexpr int kSmoothMaxFloats = 2048;  // T*C of a smooth-MPPI engine (one distribution: rollout_kernel.cuh's kMaxMeanFloats)
+
+// The smooth-MPPI merge (updateDistributionParamsFromDevice, smooth-MPPI.cu:204-240): the merged average of the rates is
+// the new rate mean, kept on the device for the next solve's K1, and the result is U = mu + dmu_new dt. mu is the nominal
+// control of the rollout being merged, carried in the parameter block.
+struct SmoothMerge
+{
+  float* rate_mean;  // [T][C]
+  float dt;
+  float mu[kSmoothMaxFloats];
+};
+
+template <bool SMOOTH>
+__device__ __forceinline__ void combine_body(const float* __restrict__ records, const float4* __restrict__ headers,
+                                             int nrec, int D, int TC, int pstride, float lambda_inv, int normalize,
+                                             float* __restrict__ out, float* __restrict__ out2, const SmoothMerge* sm)
 {
   __shared__ float scale_sh[kCombineMaxRecords];  // s_b = expf(-(beta_b - beta)/lambda)
   __shared__ float red_f[kCombineGroups];
@@ -141,7 +151,12 @@ __global__ void __launch_bounds__(kCombineCols* kCombineGroups)
     float* o2 = out2 ? out2 + (size_t)d * pstride : nullptr;
     if (col < TC)
     {
-      const float v = normalize ? a / eta_f : a;
+      float v = normalize ? a / eta_f : a;
+      if constexpr (SMOOTH)
+      {
+        sm->rate_mean[col] = v;
+        v = fmaf(v, sm->dt, sm->mu[col]);
+      }
       o[kPartialHeader + col] = v;
       if (o2)
         o2[kPartialHeader + col] = v;
@@ -161,6 +176,25 @@ __global__ void __launch_bounds__(kCombineCols* kCombineGroups)
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(kCombineCols* kCombineGroups)
+    combine_kernel(const float* __restrict__ records,   // [nrec][D][pstride]  (V at [kPartialHeader..))
+                   const float4* __restrict__ headers,  // [nrec][D] (beta_b, eta_b, sum w^2_b, -)
+                   int nrec, int D, int TC, int pstride, float lambda_inv, int normalize,
+                   float* __restrict__ out,    // [D][pstride] (device)
+                   float* __restrict__ out2)   // optional second copy (mapped host result), may be nullptr
+{
+  combine_body<false>(records, headers, nrec, D, TC, pstride, lambda_inv, normalize, out, out2, nullptr);
+}
+
+// K2 of a smooth-MPPI engine (one rank, one distribution, normalised)
+__global__ void __launch_bounds__(kCombineCols* kCombineGroups)
+    combine_kernel_smooth(const float* __restrict__ records, const float4* __restrict__ headers, int nrec, int D, int TC,
+                          int pstride, float lambda_inv, int normalize, float* __restrict__ out, float* __restrict__ out2,
+                          const __grid_constant__ SmoothMerge sm)
+{
+  combine_body<true>(records, headers, nrec, D, TC, pstride, lambda_inv, normalize, out, out2, &sm);
 }
 
 // KX — cross-GPU exchange + merge in ONE kernel over NVLink peer memory (world_size > 1, after K2 has produced this

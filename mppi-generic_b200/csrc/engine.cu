@@ -203,6 +203,11 @@ int NoiseSource::create(const mppib_desc& desc, int N, int n_offset, int n_local
   }
   if (nln)
     CUDA_TRY(nln_.alloc(noise_floats));
+  if (smooth())
+  {  // the reference leaves deriv_action_mean_d_ uninitialised (smooth-MPPI.cu:112-123); here it starts at zero
+    CUDA_TRY(rate_mean_.alloc((size_t)T * C));
+    CUDA_TRY(cudaMemsetAsync(rate_mean_, 0, (size_t)T * C * sizeof(float), stream_));
+  }
   if (colored)
   {
     // spectrum (the raw draw), time-domain buffer, tables and the reference's plan (colored_noise.cu:236-282)
@@ -319,11 +324,44 @@ int NoiseSource::seed(unsigned long long seed, unsigned long long offset)
   return MPPIB_OK;
 }
 
-void NoiseSource::burn(int n)
+// smooth-MPPI: shiftControlTrajectory at stride 1 (smooth-MPPI.cu:34-78): every row of the rate mean becomes row `row`
+__global__ void broadcast_row_kernel(float* __restrict__ a, int T, int C, int row)
+{
+  __shared__ float r[MPPIB_MAX_CONTROL_DIM];
+  if (threadIdx.x < C)
+    r[threadIdx.x] = a[row * C + threadIdx.x];
+  __syncthreads();
+  for (int i = threadIdx.x; i < T * C; i += blockDim.x)
+    a[i] = r[i % C];
+}
+
+int NoiseSource::burn(int n)
 {
   // skipping is free for a counter-positioned stream: just move the absolute offset
   rng_offset_ += (unsigned long long)n * draw_global_;  // generators are re-positioned lazily by gen_draw
   prefetch_valid_ = false;
+  // the draw chooseAppropriateKernel makes (generateSamples(1, 0, ...), mppi_controller.cu:95) shifts the rate mean too;
+  // once it is constant over t, another shift changes nothing
+  if (smooth() && n > 0)
+  {
+    broadcast_row_kernel<<<1, 256, 0, stream_>>>(rate_mean_, T_, C_, std::min(1, T_ - 1));
+    CUDA_TRY(cudaGetLastError());
+  }
+  return MPPIB_OK;
+}
+
+int NoiseSource::read_rate_mean(float* host) const
+{
+  CUDA_TRY(cudaMemcpyAsync(host, rate_mean_, (size_t)T_ * C_ * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
+}
+
+int NoiseSource::write_rate_mean(const float* host)
+{
+  CUDA_TRY(cudaMemcpyAsync(rate_mean_, host, (size_t)T_ * C_ * sizeof(float), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaStreamSynchronize(stream_));
+  return MPPIB_OK;
 }
 
 int NoiseSource::set_offset_t(long long offset_t)
@@ -599,6 +637,19 @@ int Reduction::enqueue(bool after_k1, const float* costs, const float* controls,
   return MPPIB_OK;
 }
 
+// mppib_create and mppib_set_tsallis keep a smooth engine to one rank and exponential weights
+int Reduction::enqueue_smooth(bool after_k1, float lambda, float* rate_mean, float dt, const float* mu)
+{
+  SmoothMerge m;  // 8 KB, copied into the launch's parameter block
+  m.rate_mean = rate_mean;
+  m.dt = dt;
+  memcpy(m.mu, mu, sizeof(float) * TC_);
+  CUDA_TRY(launch_on(stream_, after_k1, combine_kernel_smooth, dim3((TC_ + kCombineCols - 1) / kCombineCols, D_),
+                     dim3(kCombineCols * kCombineGroups), (const float*)partials_, (const float4*)headers_, grid_, D_, TC_,
+                     pstride_, (float)(1.0 / lambda), 1, (float*)result_, result_h_dev_, m));
+  return MPPIB_OK;
+}
+
 void Reduction::read(float* U_out, mppib_solve_stats* stats) const
 {
   for (int d = 0; d < D_; d++)
@@ -836,7 +887,9 @@ static int choose_k1(const mppib_engine& e, const PairEntry* entry, const K1Over
   const int spt = p.spt, lps = p.lps;
   // Autorally pair, one system: the warp-specialised K1 (rollout_kernel_ar_ws.cuh) — a producer and a consumer warp per 32
   // samples. MPPIB_NO_WS / MPPIB_SPW / MPPIB_SPT keep the generic kernel (A/B runs, tests of the generic form).
-  const bool ws = entry->has_warp_spec && e.D == 1 && !e.rmppi && spt == 1 && !ov.no_ws && !ov.spw_set;
+  // the smooth-MPPI sampler is built into the generic kernel only
+  p.smooth = e.noise.smooth();
+  const bool ws = entry->has_warp_spec && e.D == 1 && !e.rmppi && spt == 1 && !ov.no_ws && !ov.spw_set && !p.smooth;
   p.form = ws ? K1Form::WarpSpec
               : (e.rmppi ? K1Form::Rmppi : (e.D == 1 && spt == 2 ? K1Form::GenericSpt2 : K1Form::Generic));
   // samples per producer warp: 16 while the GPU is throughput-bound; 8 (four producers per 32 samples, one per scheduler)
@@ -1193,8 +1246,11 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
     return fail(MPPIB_ERR_INVALID_ARG, "rank out of range");
   if (desc->sampler_id == MPPIB_SAMPLER_NLN && (desc->world_size != 1 || desc->num_distributions != 1))
     return fail(MPPIB_ERR_UNSUPPORTED, "the NLN sampler is built for one rank and one distribution");
+  if (desc->sampler_id == MPPIB_SAMPLER_SMOOTH_MPPI && (desc->world_size > 1 || desc->num_distributions != 1))
+    return fail(MPPIB_ERR_UNSUPPORTED, "the smooth-MPPI sampler is built for one rank and one distribution (the reference "
+                                       "never writes the second distribution's controls, smooth-MPPI.cu:183-194)");
   if (desc->sampler_id != MPPIB_SAMPLER_GAUSSIAN && desc->sampler_id != MPPIB_SAMPLER_COLORED_NOISE &&
-      desc->sampler_id != MPPIB_SAMPLER_NLN)
+      desc->sampler_id != MPPIB_SAMPLER_NLN && desc->sampler_id != MPPIB_SAMPLER_SMOOTH_MPPI)
     return fail(MPPIB_ERR_UNSUPPORTED, "sampler %d is not built into this library", desc->sampler_id);
   if (desc->sampler_id == MPPIB_SAMPLER_COLORED_NOISE && desc->num_distributions != 1)
     return fail(MPPIB_ERR_UNSUPPORTED,
@@ -1217,6 +1273,9 @@ int mppib_create(mppib_engine** out, const mppib_desc* desc)
   bool wgmma_asked = false;
   if (int rc = Rollout::pick(*desc, &ov, &entry, &wgmma_asked))
     return rc;
+  if (desc->sampler_id == MPPIB_SAMPLER_SMOOTH_MPPI && wgmma_asked)
+    return fail(MPPIB_ERR_UNSUPPORTED, "the smooth-MPPI sampler runs on the generic rollout kernel, not the tensor-core "
+                                       "Autorally kernel (MPPIB_FLAG_NN_TENSOR)");
 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
@@ -1535,11 +1594,14 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
     return fail(MPPIB_ERR_STATE, "mppib_set_blob(%d) while a solve is pending: call mppib_solve_wait first", which);
   if (which != MPPIB_BLOB_SAMPLER_PARAMS)
     return e->model.set(which, host, nbytes);
-  if (nbytes != sizeof(mppib_gaussian_params))
-    return fail(MPPIB_ERR_INVALID_ARG, "sampler params: got %zu bytes, expected %zu", nbytes,
-                sizeof(mppib_gaussian_params));
+  const size_t expect = e->noise.smooth() ? sizeof(mppib_smooth_mppi_params) : sizeof(mppib_gaussian_params);
+  if (nbytes != expect)
+    return fail(MPPIB_ERR_INVALID_ARG, "sampler params: got %zu bytes, expected %zu", nbytes, expect);
   mppib_gaussian_params sp;
-  memcpy(&sp, host, sizeof(sp));
+  memcpy(&sp, host, sizeof(sp));  // the smooth blob begins with the Gaussian one
+  const float smooth_dt = e->noise.smooth() ? static_cast<const mppib_smooth_mppi_params*>(host)->dt : 0.0f;
+  if (!std::isfinite(smooth_dt))
+    return fail(MPPIB_ERR_INVALID_ARG, "smooth-MPPI dt must be finite");
   if (e->D > 1 && !sp.use_same_noise_for_all_distributions)
     return fail(MPPIB_ERR_UNSUPPORTED,
                 "use_same_noise_for_all_distributions = false is not supported (Tube-MPPI default is true, "
@@ -1547,7 +1609,10 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
   for (int i = 0; i < e->D * e->C; i++)
     if (!(sp.std_dev[i] > 0.0f))
       return fail(MPPIB_ERR_INVALID_ARG, "std_dev[%d] must be positive", i);
-  return e->noise.set_params(sp);
+  const int rc = e->noise.set_params(sp);
+  if (rc == MPPIB_OK && e->noise.smooth())
+    e->noise.set_smooth_dt(smooth_dt);
+  return rc;
 }
 
 int mppib_set_solver(mppib_engine* e, float dt, float lambda, float alpha)
@@ -1582,8 +1647,31 @@ int mppib_burn_draws(mppib_engine* e, int n)
 {
   if (!e || n < 0)
     return fail(MPPIB_ERR_INVALID_ARG, "bad argument");
-  e->noise.burn(n);
-  return MPPIB_OK;
+  if (e->noise.smooth())  // the burn shifts the rate mean on the device
+    CUDA_TRY(cudaSetDevice(e->desc.device));
+  return e->noise.burn(n);
+}
+
+int mppib_get_derivative_mean(mppib_engine* e, float* host)
+{
+  if (!e || !host)
+    return fail(MPPIB_ERR_INVALID_ARG, "null argument");
+  if (!e->noise.smooth())
+    return fail(MPPIB_ERR_INVALID_ARG, "only the smooth-MPPI sampler keeps a derivative (rate) mean");
+  CUDA_TRY(cudaSetDevice(e->desc.device));
+  return e->noise.read_rate_mean(host);
+}
+
+int mppib_set_derivative_mean(mppib_engine* e, const float* host)
+{
+  if (!e || !host)
+    return fail(MPPIB_ERR_INVALID_ARG, "null argument");
+  if (!e->noise.smooth())
+    return fail(MPPIB_ERR_INVALID_ARG, "only the smooth-MPPI sampler keeps a derivative (rate) mean");
+  if (e->pending != 0)
+    return fail(MPPIB_ERR_STATE, "mppib_set_derivative_mean while a solve is pending: call mppib_solve_wait first");
+  CUDA_TRY(cudaSetDevice(e->desc.device));
+  return e->noise.write_rate_mean(host);
 }
 
 int mppib_comm_unique_id(void* unique_id_128)
@@ -1648,6 +1736,24 @@ int mppib_draw_noise(mppib_engine* e)
   return MPPIB_OK;
 }
 
+// K1, and for the smooth-MPPI sampler the nominal control its merge integrates onto
+static int launch_k1(mppib_engine* e, const float* x0, const float* U_in, int optimization_stride, int iteration_num)
+{
+  if (e->noise.smooth())
+    e->smooth_mu.assign(U_in, U_in + e->TC);
+  return e->rollout.launch(*e, x0, U_in, optimization_stride, iteration_num);
+}
+
+// K2 (and its cross-rank or Tsallis stages) over the last K1's partials
+static int enqueue_merge(mppib_engine* e, bool after_k1)
+{
+  static_assert(kSmoothMaxFloats == kMaxMeanFloats, "a smooth engine's T*C is bounded by the rollout's mean");
+  if (e->noise.smooth())
+    return e->reduction.enqueue_smooth(after_k1, e->lambda, e->noise.rate_mean(), e->noise.smooth_dt(),
+                                       e->smooth_mu.data());
+  return e->reduction.enqueue(after_k1, e->rollout.costs(), e->rollout.controls(), e->n_local, e->lambda);
+}
+
 int mppib_rollout_only(mppib_engine* e, const float* x0, const float* U_in, int optimization_stride, int iteration_num)
 {
   int rc = check_ready(e);
@@ -1656,7 +1762,7 @@ int mppib_rollout_only(mppib_engine* e, const float* x0, const float* U_in, int 
   if (!x0 || !U_in)
     return fail(MPPIB_ERR_INVALID_ARG, "null argument");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = e->rollout.launch(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = launch_k1(e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -1672,7 +1778,7 @@ int mppib_reduce_only(mppib_engine* e, float* U_out, mppib_solve_stats* stats)
   if (!e->solved_once)
     return fail(MPPIB_ERR_STATE, "no rollout has been run yet");
   CUDA_TRY(cudaSetDevice(e->desc.device));
-  rc = e->reduction.enqueue(false, e->rollout.costs(), e->rollout.controls(), e->n_local, e->lambda);
+  rc = enqueue_merge(e, false);
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(cudaStreamSynchronize(e->stream));
@@ -1737,7 +1843,7 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
     return rc;
   CUDA_TRY(e->rollout.flush_l2());
   CUDA_TRY(e->timer.mark(1, e->stream));
-  rc = e->rollout.launch(*e, x0, U_in, optimization_stride, iteration_num);
+  rc = launch_k1(e, x0, U_in, optimization_stride, iteration_num);
   if (rc != MPPIB_OK)
     return rc;
   rc = e->noise.prefetch();
@@ -1745,8 +1851,7 @@ static int enqueue_solve(mppib_engine* e, const float* x0, const float* U_in, in
     return rc;
   CUDA_TRY(e->timer.mark(2, e->stream));
   // a timed solve records an event between K1 and K2: no PDL then
-  rc = e->reduction.enqueue(/*after_k1=*/!e->timer.timed(), e->rollout.costs(), e->rollout.controls(), e->n_local,
-                            e->lambda);
+  rc = enqueue_merge(e, /*after_k1=*/!e->timer.timed());
   if (rc != MPPIB_OK)
     return rc;
   CUDA_TRY(e->noise.read_by_kernel());  // K1 read it; recorded after K2, so nothing sits between K1 and PDL's K2
@@ -1841,6 +1946,8 @@ int mppib_set_tsallis(mppib_engine* e, float gamma, float r)
 {
   if (!e)
     return fail(MPPIB_ERR_INVALID_ARG, "null engine");
+  if (e->noise.smooth())
+    return fail(MPPIB_ERR_UNSUPPORTED, "Tsallis weights are not built for the smooth-MPPI sampler");
   return e->reduction.set_tsallis(gamma, r, e->rollout.controls() != nullptr);
 }
 
@@ -2073,6 +2180,8 @@ int mppib_init_eval(mppib_engine* e, const float* candidates, const int* strides
     return fail(MPPIB_ERR_INVALID_ARG, "bad argument");
   if (e->desc.world_size != 1)
     return fail(MPPIB_ERR_UNSUPPORTED, "init-eval runs on one rank (a few hundred rollouts)");
+  if (e->noise.smooth())  // RMPPI's nominal-state search; the smooth sampler is built for one distribution
+    return fail(MPPIB_ERR_UNSUPPORTED, "init-eval samples Gaussian controls; it is not built for the smooth-MPPI sampler");
   if (samples_per_candidate > e->n_local || (long)num_candidates * samples_per_candidate > e->N)
     return fail(MPPIB_ERR_INVALID_ARG, "(number of candidates) * (samples per candidate) cannot exceed NUM_ROLLOUTS");
   for (int k = 0; k < num_candidates; k++)

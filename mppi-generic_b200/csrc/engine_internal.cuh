@@ -127,6 +127,8 @@ struct mppib_engine
   Feedback feedback;  // DDP's weights, workspace and status, RMPPI's gains and value-function threshold (feedback.cuh)
   SideRollouts side;  // init-eval, sampled trajectories and the device-side roll-forward (side_rollouts.cuh)
   int pending = 0;    // solves enqueued and not yet waited for
+  // smooth-MPPI: the nominal control [T][C] of the last K1, which its merge integrates the new rate mean onto
+  std::vector<float> smooth_mu;
 
   // K1's block partials, K2 and the cross-rank merge, the result record, Tsallis weights, NCCL and KX (reduction.cuh)
   Reduction reduction;
@@ -233,6 +235,8 @@ struct Pair
 {
   using Args = RolloutArgs<DYN, COST>;
   using Kernel = void (*)(Args, CUtensorMap);
+  using SmoothArgs = SmoothRolloutArgs<DYN, COST>;
+  using SmoothKernel = void (*)(SmoothArgs, CUtensorMap);
 
   static constexpr bool kHasTensorCoreVariant = std::is_same<DYN, plugins::AutorallyNNDynamics>::value &&
                                                 std::is_same<COST, plugins::ARStandardCost>::value;
@@ -277,12 +281,26 @@ struct Pair
     fail(MPPIB_ERR_UNSUPPORTED, "this dynamics model is built for num_distributions == 1 only");
     return nullptr;
   }
-  // Sets the dynamic shared memory limit of kernel(k, stream, wb) to `smem` and, with blocks_per_sm, asks how many CTAs
-  // of `threads` threads are resident per SM. Runs in the module that holds the kernels: a plugin library links a CUDA
-  // runtime of its own, and only that one knows its kernels.
+  // The smooth-MPPI sampler's instantiation (rollout_kernel_smooth) of a generic form; choose_k1 takes no other form for it
+  static SmoothKernel smooth_kernel(const K1Plan& k, bool stream, bool wb)
+  {
+    if (k.form == K1Form::Generic)
+      return stream ? (wb ? rollout_kernel_smooth<DYN, COST, true, 1, true> : rollout_kernel_smooth<DYN, COST, false, 1, true>)
+                    : (wb ? rollout_kernel_smooth<DYN, COST, true, 1> : rollout_kernel_smooth<DYN, COST, false, 1>);
+    if (k.form == K1Form::GenericSpt2)
+    {
+      if constexpr (DYN::MAX_SPT >= 2)
+        return wb ? rollout_kernel_smooth<DYN, COST, true, 2> : rollout_kernel_smooth<DYN, COST, false, 2>;
+    }
+    fail(MPPIB_ERR_UNSUPPORTED, "the smooth-MPPI sampler runs on the generic rollout kernel only");
+    return nullptr;
+  }
+  // Sets the dynamic shared memory limit of kernel(k, stream, wb) (smooth_kernel for a smooth plan) to `smem` and, with
+  // blocks_per_sm, asks how many CTAs of `threads` threads are resident per SM. Runs in the module that holds the kernels: a
+  // plugin library links a CUDA runtime of its own, and only that one knows its kernels.
   static int kernel_attributes(const K1Plan& k, bool stream, bool wb, size_t smem, int threads, int* blocks_per_sm)
   {
-    const Kernel f = kernel(k, stream, wb);
+    const void* f = k.smooth ? (const void*)smooth_kernel(k, stream, wb) : (const void*)kernel(k, stream, wb);
     if (!f)
       return MPPIB_ERR_UNSUPPORTED;
     CUDA_TRY(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -291,12 +309,11 @@ struct Pair
     return MPPIB_OK;
   }
 
-  static int launch(mppib_engine& e, const float* x0, const float* U_in, int opt_stride, int iter)
+  // the parameter block both samplers' kernels share
+  static void fill_launch_args(Args& a, mppib_engine& e, const float* x0, const float* U_in, int opt_stride, int iter)
   {
-    static_assert(sizeof(Args) < 30000, "kernel parameter block too large");
     const Rollout& r = e.rollout;
     const K1Plan& k = r.plan();
-    Args a;
     fill_pair_args(a, e, iter);
     a.eps = e.noise.eps();
     a.costs = r.costs();
@@ -318,7 +335,33 @@ struct Pair
     a.lambda_inv = (float)(1.0 / e.lambda);  // mppi_controller.cu:201-202: 1.0 / lambda in double, narrowed
     memcpy(a.x0, x0, sizeof(float) * e.D * e.S);
     memcpy(a.means, U_in, sizeof(float) * e.D * e.TC);
+  }
+
+  static int launch(mppib_engine& e, const float* x0, const float* U_in, int opt_stride, int iter)
+  {
+    static_assert(sizeof(Args) < 30000, "kernel parameter block too large");
+    const Rollout& r = e.rollout;
+    const K1Plan& k = r.plan();
+    if (k.smooth)
+      return launch_smooth(e, x0, U_in, opt_stride, iter);
+    Args a;
+    fill_launch_args(a, e, x0, U_in, opt_stride, iter);
     kernel(k, k.stream, r.controls() != nullptr)<<<k.grid, k.threads, k.smem_bytes, e.stream>>>(
+        a, r.tensor_map(e.noise.current()));
+    CUDA_TRY(cudaGetLastError());
+    return MPPIB_OK;
+  }
+
+  static int launch_smooth(mppib_engine& e, const float* x0, const float* U_in, int opt_stride, int iter)
+  {
+    static_assert(sizeof(SmoothArgs) < 30000, "kernel parameter block too large");
+    const Rollout& r = e.rollout;
+    const K1Plan& k = r.plan();
+    SmoothArgs a;
+    fill_launch_args(a, e, x0, U_in, opt_stride, iter);
+    a.rate_mean = e.noise.rate_mean();
+    a.dt_s = e.noise.smooth_dt();
+    smooth_kernel(k, k.stream, r.controls() != nullptr)<<<k.grid, k.threads, k.smem_bytes, e.stream>>>(
         a, r.tensor_map(e.noise.current()));
     CUDA_TRY(cudaGetLastError());
     return MPPIB_OK;

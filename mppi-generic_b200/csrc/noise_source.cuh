@@ -4,6 +4,9 @@
  * A prefetched block is used only when it was drawn at the current offset, with the current sampler parameters, into a
  * buffer no kernel still reads: seed(), burn() and set_params() drop it, draw() takes it, and read_by_kernel() records
  * the kernel that the next draw into the current buffer waits for.
+ * The smooth-MPPI sampler draws as the Gaussian one does and keeps, besides, the rate mean it carries from solve to solve
+ * (device memory, zero at create): K1 reads it, the solve's merge replaces it, and burn() broadcasts its row 1, each on the
+ * solve's stream, so back-to-back solves stay in order without the host.
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -31,7 +34,7 @@ public:
   const mppib_gaussian_params& params() const { return params_; }
   bool have_params() const { return have_params_; }
   int seed(unsigned long long seed, unsigned long long offset);
-  void burn(int n);  // skip n blocks
+  int burn(int n);  // skip n blocks (smooth-MPPI: and shift the rate mean as each draw would)
   unsigned long long offset() const { return rng_offset_; }
   int set_offset_t(long long offset_t);  // optimization_stride a ColoredNoise draw assumes until a solve names its own
   int offset_t() const { return colored_offset_t_; }
@@ -46,6 +49,13 @@ public:
   bool own_kernel() const { return xw_enabled_; }
   int chunks() const { return xw_chunks_; }
   int rounds_per_chunk() const { return xw_rounds_per_chunk_; }
+  // smooth-MPPI sampler (mppib_smooth_mppi_params): the rate mean [T][C] and the sampler's dt
+  bool smooth() const { return sampler_ == MPPIB_SAMPLER_SMOOTH_MPPI; }
+  float* rate_mean() const { return rate_mean_; }
+  float smooth_dt() const { return smooth_dt_; }
+  void set_smooth_dt(float dt) { smooth_dt_ = dt; }
+  int read_rate_mean(float* host) const;   // drains the stream
+  int write_rate_mean(const float* host);  // ordered on the stream
 
 private:
   int gen_draw(int buf, cudaStream_t st, unsigned long long pos, int offset_t);
@@ -101,5 +111,8 @@ private:
   bool rearr_recorded_ = false;
   // NLN sampler: C log-normal planes + one normal block per draw (nln.cu:114-128)
   DeviceBuffer<float> nln_;  // [C][N][T]
+  // smooth-MPPI sampler
+  DeviceBuffer<float> rate_mean_;  // [T][C]
+  float smooth_dt_ = 0.015f;
 };
 }  // namespace mppib

@@ -30,6 +30,9 @@ public:
   // The merge of the partials K1 left. after_k1: K1 is the kernel just before on the stream, and K2 may start under it
   // (programmatic dependent launch). costs / controls: K1's [D][n_local] costs and written-back controls (Tsallis only).
   int enqueue(bool after_k1, const float* costs, const float* controls, int n_local, float lambda);
+  // A smooth-MPPI engine's merge (one rank, exponential weights): also writes the new rate mean rate_mean [T][C], and the
+  // result is mu + rate mean * dt
+  int enqueue_smooth(bool after_k1, float lambda, float* rate_mean, float dt, const float* mu);
   void read(float* U_out, mppib_solve_stats* stats) const;  // after the stream has drained
   int set_tsallis(float gamma, float r, bool have_controls);  // both non-zero: Tsallis weights
   int comm_init(const void* unique_id_128);

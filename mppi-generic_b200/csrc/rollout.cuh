@@ -50,6 +50,7 @@ struct K1Plan
   uint32_t smem_bytes = 0;
   bool use_tma = false;
   int dyn_shared_floats = 0;  // the dynamics' shared floats for a CTA of bx samples
+  bool smooth = false;        // the smooth-MPPI sampler's instantiation (rollout_kernel_smooth) of a generic form
 };
 
 struct K1Overrides;  // engine.cu: the descriptor flags and environment variables that choose K1's form or geometry

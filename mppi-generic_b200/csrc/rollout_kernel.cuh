@@ -26,6 +26,8 @@
  *     tile in the epilogue. Algorithmic HBM traffic = N*T*C*4 bytes (SURVEY.md §8d).
  */
 #pragma once
+#include <type_traits>
+
 #include "device_utils.cuh"
 #include "../../include/mppi_b200/params.h"
 
@@ -75,6 +77,15 @@ struct RolloutArgs
   float means[kMaxMeanFloats];                       // [D][T][C] importance-sampler mean == nominal control
 };
 
+// The smooth-MPPI sampler's K1 (SmoothMPPIDistribution, smooth-MPPI.cu): the Gaussian arguments, then the engine-held rate
+// mean and the sampler's own dt. A kernel of its own type, so that the Gaussian kernels' parameter block stays as it is.
+template <class DYN, class COST>
+struct SmoothRolloutArgs : RolloutArgs<DYN, COST>
+{
+  const float* rate_mean;  // [T][C] dmu, written by the previous solve's merge (stream order)
+  float dt_s;              // SmoothMPPIParams::dt (smooth-MPPI.cuh:21), not the controller's dt
+};
+
 // gaussian.cu:101-121: the three cases of setGaussianControls for one element
 // Branch-free: x + (-0.0f) == x for every float (including both zeros), so the pure-noise case sd * eps is the same FFMA with
 // the addend -0.0f, and the three cases become two selects instead of two divergent-branch regions per control and step.
@@ -113,7 +124,9 @@ __device__ __forceinline__ float likelihood_ratio_cost(const float* lr_scale, co
 // swizzle term (grp ^ (r & 7)) << 4 is then a per-lane constant of the unrolled body. The loads of a block are issued first and
 // unconditionally (rows past r_hi are clamped and get weight 0), so eight loads are in flight per thread instead of one
 // load-use round trip per row — when they read L2 / HBM a serialised loop would expose one memory latency per row.
-template <class DYN, class ARGS>
+// RATES (smooth-MPPI): the recomputed value is the sampled rate with mean_t = the rate mean, and it is not constrained — the
+// rate mean is the weighted average of the unconstrained rates (smooth-MPPI.cu:215-219).
+template <class DYN, class ARGS, bool RATES = false>
 __device__ __forceinline__ void weighted_control_rows(const ARGS& args, int d, int t, int row0, int r_lo, int r_hi,
                                                       const unsigned char* slab, int grp, const float* mean_t,
                                                       bool t_uses_mean, const float* wrow, bool from_global,
@@ -159,7 +172,8 @@ __device__ __forceinline__ void weighted_control_rows(const ARGS& args, int d, i
 #pragma unroll
         for (int c = 0; c < C; c++)
           u[c] = sample_control(mean_t[c], args.samp.std_dev_decayed[d][c], v[i][c], um, pn);
-        DYN::enforceConstraints(args.dyn, nullptr, u);
+        if (!RATES)
+          DYN::enforceConstraints(args.dyn, nullptr, u);
       }
       const float w = (r < r_hi) ? wrow[r] : 0.0f;
 #pragma unroll
@@ -216,10 +230,15 @@ __host__ __device__ inline RolloutSmem rollout_smem_layout(int bx, int tile_chun
 // worst it is one more read of the block's noise (C5's whole buffer, 78.6 MB, is larger than H100's 50 MB L2), against a
 // write plus a read of the same number of control bytes. Shared memory per sample drops from T*C*4 bytes to ring*128, so long horizons no longer cap the
 // block count per SM — the resident tile of C5 (T*C = 300) allows 4 warps per SM and several waves, the ring 12+ warps and one.
-template <class DYN, class COST, int D, bool WRITEBACK, int SPT, bool RMPPI = false, bool STREAM = false>
-__global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const __grid_constant__ RolloutArgs<DYN, COST> args,
-                                                      const __grid_constant__ CUtensorMap tmap)
+//
+// ARGS = SmoothRolloutArgs (rollout_kernel_smooth): the smooth-MPPI sampler. Each element's rate v is sampled around the rate
+// mean as the Gaussian sampler samples a control (the three cases of sample_control), the control is u = mu + v dt_s, and the
+// epilogue's weighted sum takes the unconstrained rates, recomputed from the noise, which the tile therefore keeps.
+template <class DYN, class COST, int D, bool WRITEBACK, int SPT, bool RMPPI, bool STREAM, class ARGS>
+__device__ __forceinline__ void rollout_body(const ARGS& args, const CUtensorMap& tmap)
 {
+  constexpr bool SMOOTH = !std::is_same<ARGS, RolloutArgs<DYN, COST>>::value;
+  static_assert(!SMOOTH || (D == 1 && !RMPPI), "smooth-MPPI is built for one distribution");
   constexpr int S = DYN::STATE_DIM, C = DYN::CONTROL_DIM, O = DYN::OUTPUT_DIM;
   static_assert(C == 1 || C == 2 || C == 4, "CONTROL_DIM must divide a 16-byte group");
   static_assert(D <= MPPIB_MAX_DISTRIBUTIONS, "too many distributions");
@@ -375,6 +394,17 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
       sd_dec[d][c] = args.samp.std_dev_decayed[d][c];
     }
   const int opt_stride = args.opt_stride;
+  // smooth-MPPI: the shift (shiftControlTrajectory, smooth-MPPI.cu:34-78) reads row min(t + s, s) in place, in t order, so
+  // every step samples around the previous rate mean's row s; a stride past the horizon takes the last row
+  float dmu[C], dt_s = 0.0f;
+  if constexpr (SMOOTH)
+  {
+    const int r = max(0, min(opt_stride, T - 1));
+#pragma unroll
+    for (int c = 0; c < C; c++)
+      dmu[c] = args.rate_mean[r * C + c];
+    dt_s = args.dt_s;
+  }
   const int ngroups = (TC + 3) >> 2;
   const uint32_t slab_bytes = (uint32_t)bx * kChunkBytes;
   unsigned char* slab = tile;
@@ -414,7 +444,13 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
         const float* mean_t = means_s + (d * T + t) * C;
 #pragma unroll
         for (int c = 0; c < C; c++)
-          u[m][c] = sample_control(mean_t[c], sd_dec[d][c], group_elem(e4[sp], s * C + c), use_mean, pure_noise[sp]);
+        {
+          if constexpr (SMOOTH)  // integrateNoise (smooth-MPPI.cu:16-32): a pure-noise row keeps mu too
+            u[m][c] = fmaf(sample_control(dmu[c], sd_dec[d][c], group_elem(e4[sp], s * C + c), use_mean, pure_noise[sp]),
+                           dt_s, mean_t[c]);
+          else
+            u[m][c] = sample_control(mean_t[c], sd_dec[d][c], group_elem(e4[sp], s * C + c), use_mean, pure_noise[sp]);
+        }
         if (RMPPI && m == 1)
         {  // fb_controller->k(x, x_nom, t) (rmppi_kernels.cu:770-784; DDP: K_t e, ddp.cu:11-45 in its host form)
 #pragma unroll
@@ -437,7 +473,7 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
             u[m][c] += ufb[c];
         }
         DYN::enforceConstraints(args.dyn, x[m], u[m]);  // mppi_common.cu:108-111
-        if (D == 1 && !STREAM)
+        if (D == 1 && !STREAM && !SMOOTH)
         {
           // single system: the constrained control replaces the noise in the shared tile (what writeControlSample does
           // in HBM, mppi_common.cu:117), so the epilogue's weighted sum reads it back instead of recomputing it
@@ -603,18 +639,37 @@ __global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const _
       // loads are in flight per thread instead of one load-use round trip per row — this loop reads L2 / HBM in the streaming
       // and RMPPI forms, where a serialised loop would expose one memory latency per row.
       const bool from_global = (RMPPI && d == 1) || STREAM;
-      const bool readback = (RMPPI && d == 1) || (STREAM && WRITEBACK && args.stream_readback);
+      const bool readback = !SMOOTH && ((RMPPI && d == 1) || (STREAM && WRITEBACK && args.stream_readback));
       const float* gsrc = readback ? args.controls_out + (size_t)d * args.n_local * T * C : args.eps;
       // the value is noise unless it comes from the constrained tile or the written-back controls: recompute the constrained
       // control (resident tile with D == 2, or the streaming variant, whose ring no longer holds it: a second read of eps
       // instead of a write + read of u)
-      weighted_control_rows<DYN>(args, d, t, row0, 0, rows_here, slab, grp, mean_t, t_uses_mean, wrow, from_global, gsrc,
-                                 !(D == 1 && !STREAM) && !readback, acc);
+      if constexpr (SMOOTH)  // the rates, around the rate mean, from the noise
+        weighted_control_rows<DYN, ARGS, true>(args, d, t, row0, 0, rows_here, slab, grp, dmu, t_uses_mean, wrow,
+                                               from_global, gsrc, true, acc);
+      else
+        weighted_control_rows<DYN>(args, d, t, row0, 0, rows_here, slab, grp, mean_t, t_uses_mean, wrow, from_global, gsrc,
+                                   !(D == 1 && !STREAM) && !readback, acc);
 #pragma unroll
       for (int c = 0; c < C; c++)
         out[col + c] = acc[c];
     }
   }
+}
+
+template <class DYN, class COST, int D, bool WRITEBACK, int SPT, bool RMPPI = false, bool STREAM = false>
+__global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS) rollout_kernel(const __grid_constant__ RolloutArgs<DYN, COST> args,
+                                                      const __grid_constant__ CUtensorMap tmap)
+{
+  rollout_body<DYN, COST, D, WRITEBACK, SPT, RMPPI, STREAM>(args, tmap);
+}
+
+// the smooth-MPPI sampler's K1: one distribution, resident or streaming, one or two samples per thread
+template <class DYN, class COST, bool WRITEBACK, int SPT, bool STREAM = false>
+__global__ void __launch_bounds__(DYN::MAX_BLOCK_THREADS)
+    rollout_kernel_smooth(const __grid_constant__ SmoothRolloutArgs<DYN, COST> args, const __grid_constant__ CUtensorMap tmap)
+{
+  rollout_body<DYN, COST, 1, WRITEBACK, SPT, false, STREAM>(args, tmap);
 }
 
 }  // namespace mppib

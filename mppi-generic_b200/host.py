@@ -34,7 +34,7 @@ DYN_RACER_SUSPENSION = 7
 COST_CARTPOLE_QUADRATIC, COST_DI_CIRCLE, COST_AR_STANDARD, COST_RACER_QUADRATIC, COST_QUADROTOR_QUADRATIC = 0, 1, 2, 3, 4
 COST_DI_ROBUST, COST_AR_ROBUST = 5, 6
 COST_QUADROTOR_MAP = 7
-SAMPLER_GAUSSIAN, SAMPLER_COLORED_NOISE, SAMPLER_NLN = 0, 1, 2
+SAMPLER_GAUSSIAN, SAMPLER_COLORED_NOISE, SAMPLER_NLN, SAMPLER_SMOOTH_MPPI = 0, 1, 2, 3
 BLOB_DYN, BLOB_COST, BLOB_SAMPLER, BLOB_NN_WEIGHTS, BLOB_COSTMAP, BLOB_LSTM_WEIGHTS, BLOB_ELEVATION_MAP = range(7)
 BLOB_COST_TEXTURE = 7
 BLOB_NORMALS_MAP = 8
@@ -348,6 +348,11 @@ class GaussianParams(C.Structure):
                 ("exponents", C.c_float * (MAX_C * MAX_D)), ("offset_decay_rate", C.c_float), ("fmin", C.c_float)]
 
 
+class SmoothMPPIParams(C.Structure):
+    """mppib_smooth_mppi_params (SmoothMPPIParams, smooth-MPPI.cuh:15-24): the Gaussian blob, then the sampler's own dt."""
+    _fields_ = [("gaussian", GaussianParams), ("dt", C.c_float)]
+
+
 class Desc(C.Structure):
     _fields_ = [("dynamics_id", C.c_int), ("cost_id", C.c_int), ("sampler_id", C.c_int), ("num_rollouts", C.c_int),
                 ("num_timesteps", C.c_int), ("num_distributions", C.c_int), ("device", C.c_int),
@@ -367,7 +372,7 @@ class Timing(C.Structure):
 # every symbol include/mppi_b200.h and include/mppi_b200/host_twins.h declare (tests check the .so exports them all)
 ABI_SYMBOLS = [
     "mppib_create", "mppib_destroy", "mppib_load_plugin", "mppib_register_pair", "mppib_set_blob", "mppib_set_solver", "mppib_seed", "mppib_burn_draws",
-    "mppib_get_rng_offset", "mppib_comm_unique_id", "mppib_comm_init", "mppib_solve", "mppib_solve_async",
+    "mppib_get_rng_offset", "mppib_get_derivative_mean", "mppib_set_derivative_mean", "mppib_comm_unique_id", "mppib_comm_init", "mppib_solve", "mppib_solve_async",
     "mppib_solve_wait", "mppib_set_option", "mppib_set_noise",
     "mppib_draw_noise", "mppib_rollout_only", "mppib_reduce_only", "mppib_get_costs", "mppib_get_noise",
     "mppib_get_samples", "mppib_get_weights", "mppib_enable_timing", "mppib_get_timing", "mppib_get_launch_info",
@@ -409,6 +414,8 @@ def lib() -> C.CDLL:
     L.mppib_seed.argtypes = [vp, C.c_ulonglong, C.c_ulonglong]
     L.mppib_burn_draws.argtypes = [vp, C.c_int]
     L.mppib_get_rng_offset.argtypes = [vp, C.POINTER(C.c_ulonglong)]
+    L.mppib_get_derivative_mean.argtypes = [vp, vp]
+    L.mppib_set_derivative_mean.argtypes = [vp, vp]
     L.mppib_comm_unique_id.argtypes = [vp]
     L.mppib_comm_init.argtypes = [vp, vp]
     L.mppib_comm_p2p_handle.argtypes = [vp, vp]
@@ -1645,6 +1652,24 @@ class NLNDistribution(GaussianDistribution):
         return np.exp(np.float32(0.5) * var), np.sqrt(np.exp(var) * np.exp(var - np.float32(1.0)))
 
 
+class SmoothMPPIDistribution(GaussianDistribution):
+    """sampling_distributions/smooth-MPPI/smooth-MPPI.cuh — samples control rates with the Gaussian parameters and
+    integrates them onto the nominal control over the sampler's own ``dt`` (default 0.015, not the controller's dt). The
+    rate mean it carries from solve to solve lives in the engine (``Engine.get_derivative_mean``). One rank, one
+    distribution."""
+    SAMPLER_ID = SAMPLER_SMOOTH_MPPI
+
+    def __init__(self, control_dim: int, std_dev: Optional[Sequence[float]] = None, dt: float = 0.015):
+        super().__init__(control_dim, std_dev)
+        self.dt = dt
+
+    def getSamplingDistributionName(self) -> str:
+        return "Smooth-MPPI"
+
+    def blob(self) -> bytes:
+        return bytes(SmoothMPPIParams(self.params, self.dt))
+
+
 # ---------------------------------------------------------------------------------------------------------------
 class Engine:
     """Thin RAII wrapper of the opaque mppib_engine (one per controller)."""
@@ -1731,6 +1756,16 @@ class Engine:
         v = C.c_ulonglong()
         _check(lib().mppib_get_rng_offset(self._h, C.byref(v)))
         return v.value
+
+    def get_derivative_mean(self) -> np.ndarray:
+        """The smooth-MPPI sampler's rate mean [T][C] (mppib_get_derivative_mean)."""
+        out = np.empty((self.T, self.Cdim), np.float32)
+        _check(lib().mppib_get_derivative_mean(self._h, _ptr(out)))
+        return out
+
+    def set_derivative_mean(self, dmu) -> None:
+        a = _f32(np.asarray(dmu, np.float32).reshape(self.T, self.Cdim))
+        _check(lib().mppib_set_derivative_mean(self._h, _ptr(a)))
 
     def comm_init(self, unique_id: bytes) -> None:
         buf = C.create_string_buffer(unique_id, 128)
