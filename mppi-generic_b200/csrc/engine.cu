@@ -37,6 +37,7 @@
 #include "rollout_kernel_nn_tc.cuh"
 #include "engine_internal.cuh"
 #include "../../include/mppi_b200/host_twins.h"
+#include "host_model.h"
 
 namespace
 {
@@ -1561,28 +1562,21 @@ int ModelParams::set(int which, const void* host, size_t nbytes)
 
 int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, float* states, float* outputs) const
 {
-  if (dyn_id_ == MPPIB_DYN_RACER_LSTM)
-  {
-    const mppib_host_lstm net{ lstm_.h.data(), dims_[0], dims_[1], nullptr, nullptr,
-                               is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr };
-    return mppib_host_output_trajectory_lstm(dyn_.data(), &net, x0, u, T, dt, states, outputs);
-  }
-  if (dyn_id_ == MPPIB_DYN_RACER_SUSPENSION_LSTM)
-  {
-    const mppib_host_lstm net{ lstm_.h.data(), dims_[0], dims_[1], nullptr, nullptr,
-                               is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr };
-    return mppib_host_output_trajectory_racer_suspension(
-        dyn_.data(), &net, is_set(MPPIB_BLOB_NORMALS_MAP) ? (const mppib_elevation_map_header*)normals_h_.data() : nullptr,
-        x0, u, T, dt, states, outputs);
-  }
-  if (dyn_id_ == MPPIB_DYN_RACER_SUSPENSION)
-    return mppib_host_output_trajectory_racer_rigid_suspension(dyn_.data(), x0, u, T, dt, states, outputs);
-  if (dyn_id_ == MPPIB_DYN_RACER_DUBINS_ELEVATION)
-    return mppib_host_output_trajectory_racer_dubins_elevation(
-        dyn_.data(), is_set(MPPIB_BLOB_ELEVATION_MAP) ? (const mppib_elevation_map_header*)elev_h_.data() : nullptr, x0, u,
-        T, dt, states, outputs);
-  return mppib_host_output_trajectory(dyn_id_, dyn_.data(), is_set(MPPIB_BLOB_NN_WEIGHTS) ? nn_.h.data() : nullptr, x0, u,
-                                      T, dt, states, outputs);
+  // a blob is set only for a model that uses it (set())
+  const auto map = [&](int which, const std::vector<unsigned char>& h) {
+    return is_set(which) ? (const mppib_elevation_map_header*)h.data() : nullptr;
+  };
+  FnnT fnn;
+  if (is_set(MPPIB_BLOB_NN_WEIGHTS))
+    fnn_transpose(nn_.h.data(), fnn);
+  const mppib_host_lstm lstm{ lstm_.h.data(), dims_[0], dims_[1], nullptr, nullptr, nullptr };
+  const HostModel m{ dyn_id_,
+                     dyn_.data(),
+                     is_set(MPPIB_BLOB_NN_WEIGHTS) ? &fnn : nullptr,
+                     is_set(MPPIB_BLOB_LSTM_WEIGHTS) ? &lstm : nullptr,
+                     map(MPPIB_BLOB_ELEVATION_MAP, elev_h_),
+                     map(MPPIB_BLOB_NORMALS_MAP, normals_h_) };
+  return roll_forward(m, x0, u, T, dt, states, outputs);
 }
 
 int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
