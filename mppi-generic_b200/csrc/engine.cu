@@ -586,6 +586,15 @@ int Reduction::create(int D, int TC, int grid, int world, int rank, cudaStream_t
   return MPPIB_OK;
 }
 
+int Reduction::set_grid(int grid)
+{
+  const size_t rec = (size_t)D_ * pstride_;
+  CUDA_TRY(partials_.reserve((size_t)grid * rec, stream_));
+  CUDA_TRY(headers_.reserve((size_t)grid * D_, stream_));
+  grid_ = grid;
+  return MPPIB_OK;
+}
+
 // What runs after the engine has drained the stream; the buffers follow.
 Reduction::~Reduction()
 {
@@ -796,7 +805,7 @@ struct mppib::K1Overrides
 // The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
 // tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
 // *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that has one, even if NN_MMA then keeps the mma.sync entry.
-int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out, bool* wgmma_asked)
+int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out, bool* wgmma_asked, bool lstm_fp16_ok)
 {
   const char* bx = getenv("MPPIB_BX");
   const char* spw = getenv("MPPIB_SPW");
@@ -841,9 +850,10 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
         entry = &p;
   }
   // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
-  // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network.
+  // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network, and so does a network
+  // whose FP16 operands would overflow (lstm_fits_fp16), where the tensor-core form would turn them into inf and NaN.
   if (entry && has_steering_lstm(desc.dynamics_id) && desc.model_dims[0] == lstm_mma::H &&
-      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt)
+      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt && lstm_fp16_ok)
     for (const auto& p : kPairsLstmMma)
       if (p.dyn_id == desc.dynamics_id && p.cost_id == desc.cost_id)
         entry = &p;
@@ -855,6 +865,54 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
                                        "not ARRobustCost");
   *out = entry;
   return MPPIB_OK;
+}
+
+// Whether the steering LSTM fits the tensor-core form's operands: lstm_mma splits every weight, pre-scaled as it loads it
+// (gates x log2 e or 2 log2 e, head layer 1 x 2 log2 e, layer 2 x -2), the initial hidden state, the hidden state and the
+// four network inputs into FP16 hi / lo halves, and a value of magnitude 65520 or more rounds to an infinite hi half,
+// which makes the products NaN. The SIMT form takes such values in FP32. So the tensor-core form is kept only when every
+// pre-scaled weight and initial hidden value, and every input bound the engine knows, is below 65504 (the largest FP16
+// value): the steering command's control range (in[2] is the clamped command), max_steer_angle * 0.2 (in[0]) and
+// max_steer_rate * 0.2 (in[3], the clamped parametric rate derivative). A blob not yet set counts as fitting; the form
+// is chosen again whenever the dynamics parameters or the weights are set (reselect_lstm_form). Out of scope: a steer rate
+// state that grows past 65504 / 0.2 at run time (in[1]), or an initial steer state outside the limits, since neither is
+// bounded by anything the engine is given. The hidden state itself stays in (-1, 1).
+static bool lstm_fits_fp16(const ModelParams& m)
+{
+  const float kMax = 65504.0f;
+  auto fits = [&](float v) { return fabsf(v) < kMax; };  // false for inf and NaN too
+  if (m.is_set(MPPIB_BLOB_DYN_PARAMS))
+  {
+    const auto* p = reinterpret_cast<const mppib_racer_lstm_dyn_params*>(m.dyn());
+    if (!fits(p->lim.rng_lo[1]) || !fits(p->lim.rng_hi[1]) || !fits(p->max_steer_angle * 0.2f) ||
+        !fits(p->max_steer_rate * 0.2f))
+      return false;
+  }
+  if (m.is_set(MPPIB_BLOB_LSTM_WEIGHTS))
+  {
+    const int H = m.dims()[0], L1 = m.dims()[1], I = MPPIB_RACER_LSTM_INPUT_DIM, HH = H * H, IH = H * I;
+    const std::vector<float>& g = m.lstm_weights_host();
+    const float sig = -lstm_mma::kLog2e, cell = 2.0f * lstm_mma::kLog2e;
+    for (int k = 0; k < 4 * HH; k++)  // W_im W_fm W_om W_cm
+      if (!fits(g[k] * (k < 3 * HH ? sig : cell)))
+        return false;
+    for (int k = 0; k < 4 * IH; k++)  // W_ii W_fi W_oi W_ci
+      if (!fits(g[4 * HH + k] * (k < 3 * IH ? sig : cell)))
+        return false;
+    const float* init_h = g.data() + 4 * HH + 4 * IH + 4 * H;
+    for (int k = 0; k < H; k++)
+      if (!fits(init_h[k]))
+        return false;
+    const float* hd = init_h + 2 * H;
+    const int IN = H + I;
+    for (int k = 0; k < L1 * IN; k++)  // W1
+      if (!fits(hd[k] * cell))
+        return false;
+    for (int k = 0; k < L1; k++)  // W2
+      if (!fits(-2.0f * hd[L1 * IN + L1 + k]))
+        return false;
+  }
+  return true;
 }
 
 // resident CTAs per SM of the generic kernel's streaming form (registers, threads and shared memory all count), for
@@ -1579,6 +1637,23 @@ int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, flo
   return roll_forward(m, x0, u, T, dt, states, outputs);
 }
 
+// The steering LSTM's form for the blobs as set now (Rollout::pick with lstm_fits_fp16): when it differs from the one K1
+// was planned for, K1 is planned again for the other entry, after the stream has drained.
+static int reselect_lstm_form(mppib_engine* e)
+{
+  K1Overrides ov;
+  const PairEntry* entry = nullptr;
+  bool wgmma_asked = false;
+  if (int rc = Rollout::pick(e->desc, &ov, &entry, &wgmma_asked, lstm_fits_fp16(e->model)))
+    return rc;
+  if (entry == &e->rollout.pair())
+    return MPPIB_OK;
+  CUDA_TRY(cudaStreamSynchronize(e->stream));
+  if (int rc = e->rollout.create(*e, entry, ov, wgmma_asked))
+    return rc;
+  return e->reduction.set_grid(e->rollout.plan().grid);
+}
+
 int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
 {
   if (!e || !host)
@@ -1587,7 +1662,12 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
   if (e->pending != 0 && ModelParams::read_by_kernels(which))
     return fail(MPPIB_ERR_STATE, "mppib_set_blob(%d) while a solve is pending: call mppib_solve_wait first", which);
   if (which != MPPIB_BLOB_SAMPLER_PARAMS)
-    return e->model.set(which, host, nbytes);
+  {
+    if (int rc = e->model.set(which, host, nbytes))
+      return rc;
+    const bool lstm_input = which == MPPIB_BLOB_DYN_PARAMS || which == MPPIB_BLOB_LSTM_WEIGHTS;
+    return lstm_input && has_steering_lstm(e->desc.dynamics_id) ? reselect_lstm_form(e) : MPPIB_OK;
+  }
   const size_t expect = e->noise.smooth() ? sizeof(mppib_smooth_mppi_params) : sizeof(mppib_gaussian_params);
   if (nbytes != expect)
     return fail(MPPIB_ERR_INVALID_ARG, "sampler params: got %zu bytes, expected %zu", nbytes, expect);

@@ -37,6 +37,7 @@ public:
   const int* dims() const { return dims_; }  // mppib_desc.model_dims
   const float* nn_weights() const { return nn_.d; }
   const float* lstm_weights() const { return lstm_.d; }
+  const std::vector<float>& lstm_weights_host() const { return lstm_.h; }
   cudaTextureObject_t costmap() const { return costmap_; }
   plugins::ElevationMap elevation_map() const { return view(elev_, MPPIB_BLOB_ELEVATION_MAP); }
   plugins::ElevationMap cost_texture() const { return view(cost_tex_, MPPIB_BLOB_COST_TEXTURE); }

@@ -23,6 +23,8 @@ public:
   // K1's per-block outputs for `grid` blocks of D distributions over T*C controls, the result record and, for world > 1,
   // the rank record and the gather buffers; the merge runs on `stream`
   int create(int D, int TC, int grid, int world, int rank, cudaStream_t stream);
+  // K1 re-planned at another grid (the steering LSTM's form chosen again): room for its partials, drained first
+  int set_grid(int grid);
   float* partials() const { return partials_; }  // [grid][D][pstride]
   float4* headers() const { return headers_; }   // [grid][D] compact (beta, eta, sum w^2)
   int pstride() const { return pstride_; }       // floats per record: the header, then T*C, rounded up to 4
