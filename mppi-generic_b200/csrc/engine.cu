@@ -805,7 +805,7 @@ struct mppib::K1Overrides
 // The pair entry for the descriptor: the built-in or registered pair, or the Autorally pair's mma.sync form and the LSTM's
 // tensor-core form unless an override keeps the other. Needs no device, so these refusals come before any device work.
 // *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that has one, even if NN_MMA then keeps the mma.sync entry.
-int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out, bool* wgmma_asked, bool lstm_fp16_ok)
+int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out, bool* wgmma_asked, bool fp16_ok)
 {
   const char* bx = getenv("MPPIB_BX");
   const char* spw = getenv("MPPIB_SPW");
@@ -838,8 +838,9 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
       entry = p;
   *wgmma_asked = entry && entry->has_wgmma && o.nn_tensor;
   // Autorally pair: the network runs on register-level mma.sync by default (plugins/nn_mma.cuh). NN_FFMA2 keeps the FFMA2
-  // form, NN_TENSOR selects the wgmma kernel (which is built on the FFMA2 entry).
-  if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(o.nn_ffma2 || o.nn_tensor) || o.nn_mma))
+  // form, NN_TENSOR selects the wgmma kernel (which is built on the FFMA2 entry). A network whose FP16 operands would
+  // overflow (network_fits_fp16) keeps the FFMA2 entry even under NN_MMA: mma.sync would turn them into inf and NaN.
+  if (entry && desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN && (!(o.nn_ffma2 || o.nn_tensor) || o.nn_mma) && fp16_ok)
   {
     // samples per warp of the generic kernel's network (plugins/nn_mma.cuh): 32. Narrower sample groups (MPPIB_SPW = 16 / 8)
     // halve / quarter a warp's tensor work per step, but the step time of a lone warp barely moves: the chain, not the
@@ -851,9 +852,9 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
   }
   // steering LSTM at hidden_dim 32 (head width <= 24): gates and head as mma.sync products, hidden / cell state in fragment
   // layout in registers (plugins/lstm_mma.cuh). LSTM_SIMT keeps the one-thread-per-sample network, and so does a network
-  // whose FP16 operands would overflow (lstm_fits_fp16), where the tensor-core form would turn them into inf and NaN.
+  // whose FP16 operands would overflow (network_fits_fp16), where the tensor-core form would turn them into inf and NaN.
   if (entry && has_steering_lstm(desc.dynamics_id) && desc.model_dims[0] == lstm_mma::H &&
-      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt && lstm_fp16_ok)
+      desc.model_dims[1] <= 8 * lstm_mma::kHeadTiles && !o.lstm_simt && fp16_ok)
     for (const auto& p : kPairsLstmMma)
       if (p.dyn_id == desc.dynamics_id && p.cost_id == desc.cost_id)
         entry = &p;
@@ -867,20 +868,50 @@ int Rollout::pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** out
   return MPPIB_OK;
 }
 
-// Whether the steering LSTM fits the tensor-core form's operands: lstm_mma splits every weight, pre-scaled as it loads it
-// (gates x log2 e or 2 log2 e, head layer 1 x 2 log2 e, layer 2 x -2), the initial hidden state, the hidden state and the
-// four network inputs into FP16 hi / lo halves, and a value of magnitude 65520 or more rounds to an infinite hi half,
-// which makes the products NaN. The SIMT form takes such values in FP32. So the tensor-core form is kept only when every
-// pre-scaled weight and initial hidden value, and every input bound the engine knows, is below 65504 (the largest FP16
-// value): the steering command's control range (in[2] is the clamped command), max_steer_angle * 0.2 (in[0]) and
-// max_steer_rate * 0.2 (in[3], the clamped parametric rate derivative). A blob not yet set counts as fitting; the form
-// is chosen again whenever the dynamics parameters or the weights are set (reselect_lstm_form). Out of scope: a steer rate
-// state that grows past 65504 / 0.2 at run time (in[1]), or an initial steer state outside the limits, since neither is
-// bounded by anything the engine is given. The hidden state itself stays in (-1, 1).
-static bool lstm_fits_fp16(const ModelParams& m)
+// Whether the model's network fits its tensor-core form's FP16 operands. Both forms split every operand into FP16 hi / lo
+// halves (plugins/nn_mma.cuh, plugins/lstm_mma.cuh: split2), and a value of magnitude 65520 or more rounds to an infinite
+// hi half, which makes the products NaN; the FP32 forms (FFMA2, SIMT) take such values as they are. So the FP16 form is
+// kept only when every pre-scaled weight, and every input bound the engine knows, is below 65504 (the largest FP16
+// value). A blob not yet set counts as fitting; the form is chosen again whenever the dynamics parameters or the weights
+// are set (reselect_network_form). Biases need no check: both forms keep them in FP32 (C fragments). Models without an
+// FP16 form always fit.
+//  * Steering LSTM: the gate weights (x -log2 e, or 2 log2 e for the cell gate), head layer 1 (x 2 log2 e) and layer 2
+//    (x -2), the initial hidden state, and the input bounds: the steering command's control range (in[2] is the clamped
+//    command), max_steer_angle * 0.2 (in[0]) and max_steer_rate * 0.2 (in[3], the clamped parametric rate derivative).
+//    Out of scope: a steer rate state that grows past 65504 / 0.2 at run time (in[1]), or an initial steer state outside
+//    the limits, since neither is bounded by anything the engine is given. The hidden state itself stays in (-1, 1).
+//  * Autorally network (nn_mma::load_weights): W1 x 2 log2 e, W2 x -4 log2 e, W3 x -2, and both control ranges (in[4],
+//    in[5] are the clamped commands). Out of scope: states (roll, speeds, yaw rate) that grow past 65504 at run time.
+static bool network_fits_fp16(const mppib_desc& desc, const ModelParams& m)
 {
   const float kMax = 65504.0f;
   auto fits = [&](float v) { return fabsf(v) < kMax; };  // false for inf and NaN too
+  if (desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN)
+  {
+    if (m.is_set(MPPIB_BLOB_DYN_PARAMS))
+    {
+      const auto& lim = reinterpret_cast<const mppib_ar_nn_dyn_params*>(m.dyn())->lim;
+      for (int c = 0; c < 2; c++)
+        if (!fits(lim.rng_lo[c]) || !fits(lim.rng_hi[c]))
+          return false;
+    }
+    if (m.is_set(MPPIB_BLOB_NN_WEIGHTS))
+    {
+      const std::vector<float>& g = m.nn_weights_host();
+      for (int k = 0; k < 192; k++)  // W1
+        if (!fits(g[k] * nn_mma::kTanhScale))
+          return false;
+      for (int k = 224; k < 1248; k++)  // W2
+        if (!fits(g[k] * (-2.0f * nn_mma::kTanhScale)))
+          return false;
+      for (int k = 1280; k < 1408; k++)  // W3
+        if (!fits(g[k] * -2.0f))
+          return false;
+    }
+    return true;
+  }
+  if (!has_steering_lstm(desc.dynamics_id))
+    return true;
   if (m.is_set(MPPIB_BLOB_DYN_PARAMS))
   {
     const auto* p = reinterpret_cast<const mppib_racer_lstm_dyn_params*>(m.dyn());
@@ -1637,14 +1668,15 @@ int ModelParams::host_roll(const float* x0, const float* u, int T, float dt, flo
   return roll_forward(m, x0, u, T, dt, states, outputs);
 }
 
-// The steering LSTM's form for the blobs as set now (Rollout::pick with lstm_fits_fp16): when it differs from the one K1
-// was planned for, K1 is planned again for the other entry, after the stream has drained.
-static int reselect_lstm_form(mppib_engine* e)
+// The network's form for the blobs as set now (Rollout::pick with network_fits_fp16): when it differs from the one K1 was
+// planned for, K1 is planned again for the other entry, after the stream has drained. The side rollouts and DDP follow
+// the entry.
+static int reselect_network_form(mppib_engine* e)
 {
   K1Overrides ov;
   const PairEntry* entry = nullptr;
   bool wgmma_asked = false;
-  if (int rc = Rollout::pick(e->desc, &ov, &entry, &wgmma_asked, lstm_fits_fp16(e->model)))
+  if (int rc = Rollout::pick(e->desc, &ov, &entry, &wgmma_asked, network_fits_fp16(e->desc, e->model)))
     return rc;
   if (entry == &e->rollout.pair())
     return MPPIB_OK;
@@ -1665,8 +1697,10 @@ int mppib_set_blob(mppib_engine* e, int which, const void* host, size_t nbytes)
   {
     if (int rc = e->model.set(which, host, nbytes))
       return rc;
-    const bool lstm_input = which == MPPIB_BLOB_DYN_PARAMS || which == MPPIB_BLOB_LSTM_WEIGHTS;
-    return lstm_input && has_steering_lstm(e->desc.dynamics_id) ? reselect_lstm_form(e) : MPPIB_OK;
+    const bool net_input = which == MPPIB_BLOB_DYN_PARAMS || which == MPPIB_BLOB_LSTM_WEIGHTS ||
+                           which == MPPIB_BLOB_NN_WEIGHTS;
+    const bool has_fp16_form = has_steering_lstm(e->desc.dynamics_id) || e->desc.dynamics_id == MPPIB_DYN_AUTORALLY_NN;
+    return net_input && has_fp16_form ? reselect_network_form(e) : MPPIB_OK;
   }
   const size_t expect = e->noise.smooth() ? sizeof(mppib_smooth_mppi_params) : sizeof(mppib_gaussian_params);
   if (nbytes != expect)

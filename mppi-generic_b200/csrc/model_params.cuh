@@ -36,6 +36,7 @@ public:
   const unsigned char* cost() const { return cost_.data(); }
   const int* dims() const { return dims_; }  // mppib_desc.model_dims
   const float* nn_weights() const { return nn_.d; }
+  const std::vector<float>& nn_weights_host() const { return nn_.h; }
   const float* lstm_weights() const { return lstm_.d; }
   const std::vector<float>& lstm_weights_host() const { return lstm_.h; }
   cudaTextureObject_t costmap() const { return costmap_; }

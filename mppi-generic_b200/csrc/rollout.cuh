@@ -59,10 +59,10 @@ class Rollout : NoCopy
 {
 public:
   // The pair entry for the descriptor and the overrides; *wgmma_asked: NN_TENSOR asks for the wgmma kernel of a pair that
-  // has one. lstm_fp16_ok: the steering LSTM's weights and known input bounds fit the tensor-core form's FP16 operands
-  // (engine.cu: lstm_fits_fp16). Needs no device.
+  // has one. fp16_ok: the model's network (steering LSTM or Autorally) and its known input bounds fit the FP16 operands of
+  // its mma.sync form (engine.cu: network_fits_fp16). Needs no device.
   static int pick(const mppib_desc& desc, K1Overrides* ov, const PairEntry** entry, bool* wgmma_asked,
-                  bool lstm_fp16_ok = true);
+                  bool fp16_ok = true);
   // After the engine's sizes, flags and SM count are set and its noise source is created: the plan, write-back, the
   // buffers, the tensor maps and the kernel's attributes
   int create(const mppib_engine& e, const PairEntry* entry, const K1Overrides& ov, bool wgmma_asked);
